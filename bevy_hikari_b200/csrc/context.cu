@@ -93,6 +93,7 @@ struct hk_context {
     uint8_t* noise = nullptr;
     Counters* counters = nullptr;
     SpatialTable* spatial_tables = nullptr;
+    SpatialTable spatial_tables_host[2];  // the same two tables on the host: kc_spatial takes its table as a kernel parameter
     bool count_rays = false, time_passes = false, keep_intermediates = false;
     bool pooled_indirect = HK_POOLED_INDIRECT != 0;   // hk_set_tuning(HK_TUNE_POOLED_INDIRECT)
     bool tiled_denoise = true;                        // hk_set_tuning(HK_TUNE_TILED_DENOISE): kc_denoise (TMA tiles) vs k_denoise (gathers)
@@ -352,6 +353,7 @@ int hk_context_create_tile(hk_context** out, int cuda_device, uint32_t width, ui
                 }
             }
         }
+        memcpy(c->spatial_tables_host, t, sizeof(t));
         void* p = nullptr;
         if (cudaMalloc(&p, sizeof(t)) != cudaSuccess) rc = set_error(c, HK_ERR_OUT_OF_MEMORY, "spatial tables");
         else {
@@ -1055,7 +1057,7 @@ static int ring_of(const KParams& P) { return P.tile_images ? RING_TONE : 0; }  
 static void launch_spatial(hk_context* ctx, const KParams& P, bool emissive) {
     const int v = emissive ? 1 : 0, parity = 1 - (int)(P.in.frame.number & 1u);
     const bool tiled = ctx->tile_maps_ready && ctx->tiled_spatial;
-    hk_launch_spatial(P, emissive, tiled ? &ctx->tm_depth[v] : nullptr, tiled ? &ctx->tm_q3[v][parity] : nullptr, ctx->stream);
+    hk_launch_spatial(P, emissive, tiled ? &ctx->tm_depth[v] : nullptr, tiled ? &ctx->tm_q3[v][parity] : nullptr, ctx->spatial_tables_host[v], ctx->stream);
 }
 static const TileMap* denoise_maps(hk_context* ctx, int level) { return (ctx->tile_maps_ready && ctx->tiled_denoise) ? ctx->tm_denoise[level] : nullptr; }
 static int run_light(hk_context* ctx, KParams& P) {  // LightNode::run order, light.rs:645-699 (albedo is fused in the prepass)

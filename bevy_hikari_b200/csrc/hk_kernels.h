@@ -10,7 +10,8 @@ void hk_launch_direct(const hkd::KParams& P, bool emissive, bool count, bool wid
 void hk_launch_indirect(const hkd::KParams& P, bool multi, bool count, bool wide, cudaStream_t st);
 // pooled (cooperative) form of the indirect pass: shared-memory ray pool, dynamic fetch, TMA-staged scene records (kernels_pool.cu)
 void hk_launch_indirect_pool(const hkd::KParams& P, bool multi, bool count, cudaStream_t st);
-void hk_launch_spatial(const hkd::KParams& P, bool emissive, const hkd::TileMap* depth_map, const hkd::TileMap* q3_map, cudaStream_t st);
+void hk_launch_spatial(const hkd::KParams& P, bool emissive, const hkd::TileMap* depth_map, const hkd::TileMap* q3_map, const hkd::SpatialTable& table,
+                       cudaStream_t st);
 void hk_launch_extract_depth(const hkd::KParams& P, cudaStream_t st);   // depth plane <- pos_depth.w over the launch rectangle
 void hk_launch_scatter_resolve(const hkd::KParams& P, int signal, cudaStream_t st);
 void hk_launch_trace_rays(const hkd::DeviceScene& sc, const hk_ray* rays, size_t n, hk_hit* hits, bool wide, cudaStream_t st);

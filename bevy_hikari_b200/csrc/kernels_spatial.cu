@@ -17,13 +17,22 @@
 #define HK_SPATIAL_FAST_DIV 1
 #endif
 
-// CTAs of 256 threads per SM of the tiled kernel: 66 KB of tiles each for the indirect pipeline (at most 3 fit), 28 KB for the emissive one.
-// 2 CTAs/SM = 126 registers without spills rather than 3 CTAs/SM = 80 registers with spills for the indirect pipeline
+// CTAs of 256 threads per SM of the tiled kernel: 74 KB of shared memory each for the indirect pipeline (at most 3 fit), 32 KB for the
+// emissive one.  2 CTAs/SM = 127 registers without spills rather than 3 CTAs/SM = 80 registers with spills (slower on the H100)
 #ifndef HK_SPATIAL_TILED_MINB_INDIRECT
 #define HK_SPATIAL_TILED_MINB_INDIRECT 2
 #endif
 #ifndef HK_SPATIAL_TILED_MINB_EMISSIVE
 #define HK_SPATIAL_TILED_MINB_EMISSIVE 2
+#endif
+// kc_spatial stages its tiles only when one of its pixels is a surface pixel (=0: every CTA stages them, for A/B runs)
+#ifndef HK_SPATIAL_SKIP_EMPTY_TILES
+#define HK_SPATIAL_SKIP_EMPTY_TILES 1
+#endif
+// Surviving neighbours whose gathers kc_spatial keeps in flight ahead of the one it merges.  Each holds 12 registers: 2 spills at the
+// 127-register cap of 2 CTAs/SM and was slower on the H100 (cornell 1080p)
+#ifndef HK_SPATIAL_GATHER_AHEAD
+#define HK_SPATIAL_GATHER_AHEAD 1
 #endif
 
 namespace hkd {
@@ -181,16 +190,46 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_SPATIAL) k_spatial(const 
 }
 
 
+// Frame pixel (tx, ty) of tap j (1-based) of neighbour i's screen-space depth march (light.wgsl:1608-1628) at upscale ratio 1
+__device__ __forceinline__ void march_tap(const KParams& P, const SpatialTable& T, uint32_t i, uint32_t j, vec2 uv, vec2 size_f, vec2 unit,
+                                          int& tx, int& ty) {
+    float tap_dist = T.tap_dist[i][j - 1u];
+#if HK_SPATIAL_FAST_DIV
+    const vec2 tap_offset = tap_dist * unit;
+    const float qx = tap_offset.x * P.inv_rw, qy = tap_offset.y * P.inv_rh;
+    vec2 tap_uv = uv + v2(fmaf(fmaf(-qx, size_f.x, tap_offset.x), P.inv_rw, qx), fmaf(fmaf(-qy, size_f.y, tap_offset.y), P.inv_rh, qy));
+#else
+    vec2 tap_uv = uv + (tap_dist * unit) / size_f;
+#endif
+    tx = f32_to_i32(tap_uv.x * (float)P.band.W); ty = f32_to_i32(tap_uv.y * (float)P.band.H);
+}
+// The depth march of neighbour i with every tap read from the G-buffer instead of the staged tile: kc_spatial's fallback when a tap
+// lies in the frame but outside the tile (a tap lies between the pixel and its neighbour, hence inside it; a float coordinate that
+// rounds one pixel out of it has never been observed) or when the table holds more taps than kc_spatial unrolls
+static __device__ HK_NOINLINE bool march_occluded_from_plane(const KParams& P, const SpatialTable& T, uint32_t i, vec2 uv, vec2 size_f,
+                                                              vec2 unit, float depth, float sample_depth) {
+    for (uint32_t j = 1u; j <= T.tap_count[i]; j += 1u) {
+        int tx, ty;
+        march_tap(P, T, i, j, uv, size_f, unit, tx, ty);
+        float tap_depth = 0.0f;  // out-of-bounds textureLoad -> 0
+        if (tx >= 0 && tx < P.band.W && ty >= 0 && ty < P.band.H) tap_depth = P.planes.pos_depth[band_index(P.band, tx, ty)].w;
+        if (tap_depth > mixf(depth, sample_depth, T.tap_ratio[i][j - 1u]) + 0.00001f) return true;
+    }
+    return false;
+}
+
 // ------------------------------------------------------------------------- P4 with TMA-staged neighbourhood tiles
 // kc_spatial: the same pass for upscale ratio 1 (render space == G-buffer space: every benchmark and every tiled configuration).
 // A CTA of 16 x 16 pixels stages, with two TMA tile loads (cp.async.bulk.tensor.2d, hk_tile.cuh), the part of the frame its
 // neighbours can lie in — its own tile grown by the reuse radius (20 px indirect, 10 px emissive):
 //   * the G-buffer depth plane                          (4 B / px):  the neighbour's depth and every tap of the depth march
 //   * quarter 3 of the temporal reservoir being reused (16 B / px):  count + visible normal, i.e. the cheap rejections
-// 60 x 56 x 20 B = 66 KB (indirect) / 40 x 36 x 20 B = 28 KB (emissive) of shared memory.  Per pixel that replaces 16 (8) scattered
-// depth fetches, up to 80 (40) scattered depth-march taps and the 64-byte reservoir fetches of the neighbours that the depth, count
-// and normal tests reject by reads from shared memory; the three remaining quarters of a surviving neighbour are requested together.
-// Arithmetic, test order within a neighbour and merge order are those of k_spatial: same bytes out (exact flavour).
+// 60 x 56 x 20 B = 66 KB (indirect) / 40 x 36 x 20 B = 28 KB (emissive) of shared memory, plus 2 bytes per neighbour and thread for
+// the hand-over between the two stages below.  Per pixel that replaces 16 (8) scattered depth fetches, up to 80 (40) scattered
+// depth-march taps and the 64-byte reservoir fetches of the neighbours that the depth, count, normal and march tests reject by reads
+// from shared memory.  Stage A runs those tests for every neighbour; stage B gathers the three remaining quarters of the survivors
+// only (about 9 of 16 indirect and 5 of 8 emissive neighbours of a surface pixel on cornell 1080p) and merges them.
+// Arithmetic and merge order are those of k_spatial: same bytes out (exact flavour).
 template <bool EMISSIVE_LIT> struct SpatialTile {
     static constexpr int R = EMISSIVE_LIT ? 10 : 20;
     static constexpr int BH = POOL_TILE_H + 2 * R;                    // rows of the neighbourhood
@@ -198,12 +237,15 @@ template <bool EMISSIVE_LIT> struct SpatialTile {
     // every TMA destination starts on a 128-byte boundary
     static constexpr size_t DEPTH_BYTES = ((size_t)BW * BH * 4 + 127) & ~(size_t)127, Q3_BYTES = ((size_t)BW * BH * 16 + 127) & ~(size_t)127;
     static constexpr uint32_t TX_BYTES = (uint32_t)((size_t)BW * BH * 20);     // what the two copies deliver
-    static constexpr size_t SMEM_BYTES = DEPTH_BYTES + Q3_BYTES + 16;       // + the mbarrier
+    static constexpr uint32_t COUNT = EMISSIVE_LIT ? 8u : 16u;
+    static constexpr size_t CELL_BYTES = (size_t)COUNT * POOL_THREADS * 2;    // stage A -> B: each survivor's cell, u16 per neighbour and thread
+    static constexpr size_t SMEM_BYTES = DEPTH_BYTES + Q3_BYTES + CELL_BYTES + 16;       // + the mbarrier
+    static_assert((size_t)BW * BH <= 65536, "cells fit in 16 bits");
 };
 
 template <bool EMISSIVE_LIT, bool TEX = true>
 __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_MINB_EMISSIVE : HK_SPATIAL_TILED_MINB_INDIRECT) kc_spatial(const __grid_constant__ KParams P, const __grid_constant__ TileMap depth_map,
-                                                                                   const __grid_constant__ TileMap q3_map) {
+                                                                                   const __grid_constant__ TileMap q3_map, const __grid_constant__ SpatialTable T) {
     using ST = SpatialTile<EMISSIVE_LIT>;
     constexpr int SIGNAL = EMISSIVE_LIT ? 1 : 2;
     constexpr uint32_t SPATIAL_REUSE_COUNT = EMISSIVE_LIT ? 8u : 16u;   // light.wgsl:246-252
@@ -211,18 +253,22 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
     HK_DYNAMIC_SMEM(smem);
     float* s_depth = reinterpret_cast<float*>(smem);
     uint4* s_q3 = reinterpret_cast<uint4*>(smem + ST::DEPTH_BYTES);
-    uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem + ST::DEPTH_BYTES + ST::Q3_BYTES);
+    uint16_t* s_cell = reinterpret_cast<uint16_t*>(smem + ST::DEPTH_BYTES + ST::Q3_BYTES);
+    uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem + ST::DEPTH_BYTES + ST::Q3_BYTES + ST::CELL_BYTES);
     // tile origin in frame coordinates, and in plane (allocation) coordinates for the copy engine
     const int px0 = tile_origin_x(P.col_lo + (int)blockIdx.x * POOL_TILE_W - R - P.band.ax0);       // plane column of the tile's first cell
     const int tx0 = px0 + P.band.ax0, ty0 = P.row_lo + (int)blockIdx.y * POOL_TILE_H - R;
-    if (threadIdx.x == 0) {
-        mbar_init(s_bar, 1u);
+    auto stage_tiles = [&]() {
         mbar_expect_tx(s_bar, ST::TX_BYTES);
         tile_load_2d(s_depth, &depth_map, px0, ty0 - P.band.a0, s_bar);
         tile_load_2d(s_q3, &q3_map, 4 * px0, ty0 - P.band.a0, s_bar);      // the plane as rows of u32: 4 per pixel
         mbar_complete_emulated(s_bar);
+    };
+    if (threadIdx.x == 0) {
+        mbar_init(s_bar, 1u);
+        if (!HK_SPATIAL_SKIP_EMPTY_TILES) stage_tiles();
     }
-    __syncthreads();                                    // the barrier is initialised before anybody waits on it
+    if (!HK_SPATIAL_SKIP_EMPTY_TILES) __syncthreads();      // the barrier is initialised before anybody waits on it
 
     int x, y;
     pool_pixel(x, y, P);
@@ -242,7 +288,15 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
         store_quarters(Bf.spatial_reservoir, idx, pack_reservoir(unpack_reservoir(own)));
         P.planes.render[SIGNAL][idx] = make_uint2(0u, 0u);
     }
+#if HK_SPATIAL_SKIP_EMPTY_TILES
+    // A CTA of background pixels only (around the model) needs no neighbourhood: it stages nothing and leaves at once.  Otherwise
+    // its background threads leave without waiting: the surface threads wait for the copies before the CTA's memory can go away.
+    if (!__syncthreads_or(surface_pixel)) return;       // (also orders the barrier's initialisation before any wait on it)
+    if (threadIdx.x == 0) stage_tiles();
+    if (!surface_pixel) return;
+#else
     if (!surface_pixel) { mbar_wait(s_bar, 0u); return; }      // (every thread observes the copies before the CTA's memory can go away)
+#endif
 
     Reservoir r = unpack_reservoir(own);
     const ShadeEnv env = make_env(P);
@@ -274,77 +328,87 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
     r.s.visible_normal = s.visible_normal;
 
     const vec2 size_f = v2((float)P.band.RW, (float)P.band.RH);
-    const SpatialTable& T = P.spatial_tables[EMISSIVE_LIT ? 1 : 0];
     const float rotation = sum4(s.random);
     mbar_wait(s_bar, 0u);                               // the tiles have landed
-    // The neighbours are software-pipelined by one: while neighbour i is unpacked, marched and shaded, the cheap tests of neighbour
-    // i + 1 (shared memory only) have already run and its three remaining quarters are in flight — one exposed L2 latency per pixel
-    // instead of one per surviving neighbour.  Order of the merges, and every value, unchanged.
-    struct Candidate { bool valid; vec2 offset; float sample_depth; uint4 q0, q1, q2, q3; };
-    auto prepare = [&](uint32_t i) -> Candidate {
-        Candidate c;
-        c.valid = false; c.offset = v2(0.0f, 0.0f); c.sample_depth = 0.0f;
-        c.q0 = c.q1 = c.q2 = c.q3 = make_uint4(0u, 0u, 0u, 0u);
-        if (i > SPATIAL_REUSE_COUNT) return c;
+
+    // Stage A, shared memory only: every test that rejects a neighbour without its gathered quarters — bounds, depth ratio, count
+    // and visible normal (staged quarter 3) and the screen-space depth march (light.wgsl:1608-1628).  The march runs before the
+    // hemisphere test of stage B instead of after it: every test is a pure rejection, so the set of merged neighbours is the same.
+    // Unrolled, so that the independent neighbours' shared-memory chains interleave.  Each survivor's cell goes to s_cell.
+    uint32_t survivors = 0u;                            // bit i: neighbour i passed stage A
+#pragma unroll
+    for (uint32_t i = 1u; i <= SPATIAL_REUSE_COUNT; i += 1u) {
         float ang = TAU * fract(T.phase[i] + rotation + P.random_frame);
         const float rad = T.radius[i];
         float sn, cs;
         sincos_(ang, &sn, &cs);
-        c.offset = rad * v2(cs, sn);
-        int sx = f32_to_i32(c.offset.x + (float)x), sy = f32_to_i32(c.offset.y + (float)y);
-        if (sx < 0 || sy < 0 || sx >= P.band.RW || sy >= P.band.RH) return c;      // see k_spatial
+        const vec2 offset = rad * v2(cs, sn);
+        int sx = f32_to_i32(offset.x + (float)x), sy = f32_to_i32(offset.y + (float)y);
+        if (sx < 0 || sy < 0 || sx >= P.band.RW || sy >= P.band.RH) continue;      // see k_spatial
         const int tcell = (sy - ty0) * BW + (sx - tx0);
-        c.sample_depth = s_depth[tcell];
-        float depth_ratio = depth / c.sample_depth;
-        if (depth_ratio < 0.9f || depth_ratio > 1.1f) return c;
-        // count and visible normal from the staged quarter: the same values unpack_reservoir derives from it below
-        c.q3 = s_q3[tcell];
-        const float n_count = unpack2x16float(c.q3.z).x;
-        const vec3 n_normal = normalize(xyz(unpack4x8snorm(c.q3.x)));
-        if (n_count < F32_EPSILON || dot(s.visible_normal, n_normal) < 0.866f) return c;
-        const size_t sidx = render_index(P.band, sx, sy);
-        c.q0 = __ldg(&Bf.reservoir.q[0][sidx]); c.q1 = __ldg(&Bf.reservoir.q[1][sidx]); c.q2 = __ldg(&Bf.reservoir.q[2][sidx]);
-        c.valid = true;
-        return c;
+        const float sample_depth = s_depth[tcell];
+        float depth_ratio = depth / sample_depth;
+        if (depth_ratio < 0.9f || depth_ratio > 1.1f) continue;
+        // count and visible normal from the staged quarter: the same values unpack_reservoir derives from it in stage B
+        const uint4 n_q3 = s_q3[tcell];
+        const float n_count = unpack2x16float(n_q3.z).x;
+        const vec3 n_normal = normalize(xyz(unpack4x8snorm(n_q3.x)));
+        if (n_count < F32_EPSILON || dot(s.visible_normal, n_normal) < 0.866f) continue;
+
+        // screen-space depth march towards the neighbour, every tap out of the staged depth tile.  No exit at the first occluding tap
+        // and no branch per tap: "some tap lies in front" is the same outcome, and the taps' shared-memory reads overlap instead of
+        // forming a chain of dependent reads and branches (the march was the costliest part of the pass).  tap_count <= 5:
+        // u32(radius / max(1, radius / 5)).
+        const uint32_t tap_count = T.tap_count[i];
+        bool occluded = false, from_plane = tap_count > 5u;
+        vec2 unit = normalize(offset);
+#pragma unroll
+        for (uint32_t j = 1u; j <= 5u; j += 1u) {
+            int tx, ty;
+            march_tap(P, T, i, j, uv, size_f, unit, tx, ty);
+            const bool in_frame = tx >= 0 && tx < P.band.W && ty >= 0 && ty < P.band.H;      // out-of-bounds textureLoad -> 0
+            const int cxl = tx - tx0, cyl = ty - ty0;
+            const bool in_tile = (unsigned)cxl < (unsigned)BW && (unsigned)cyl < (unsigned)BH;
+            const float staged = s_depth[in_tile ? cyl * BW + cxl : 0];
+            const float tap_depth = in_frame ? staged : 0.0f;
+            const bool live = j <= tap_count;
+            from_plane |= live && in_frame && !in_tile;
+            occluded |= live && tap_depth > mixf(depth, sample_depth, T.tap_ratio[i][j - 1u]) + 0.00001f;
+        }
+        if (from_plane) occluded = march_occluded_from_plane(P, T, i, uv, size_f, unit, depth, sample_depth);
+        if (occluded) continue;
+        survivors |= 1u << i;
+        s_cell[(i - 1u) * POOL_THREADS + threadIdx.x] = (uint16_t)tcell;
+    }
+
+    // Stage B, survivors only, in neighbour order: the three quarters not staged are gathered from the planes while the survivor
+    // before them is unpacked, tested against the hemisphere and merged.  Rejected neighbours no longer sit between two gathers.
+    struct Gather { bool valid; int cell; uint4 q0, q1, q2; };
+    auto gather_next = [&]() -> Gather {
+        Gather g;
+        g.valid = survivors != 0u; g.cell = 0;
+        g.q0 = g.q1 = g.q2 = make_uint4(0u, 0u, 0u, 0u);
+        if (!g.valid) return g;
+        const uint32_t i = (uint32_t)__ffs(survivors) - 1u;
+        survivors &= survivors - 1u;
+        g.cell = s_cell[(i - 1u) * POOL_THREADS + threadIdx.x];
+        const size_t sidx = render_index(P.band, tx0 + g.cell % BW, ty0 + g.cell / BW);
+        g.q0 = __ldg(&Bf.reservoir.q[0][sidx]); g.q1 = __ldg(&Bf.reservoir.q[1][sidx]); g.q2 = __ldg(&Bf.reservoir.q[2][sidx]);
+        return g;
     };
-    Candidate next = prepare(1u);
-    for (uint32_t i = 1u; i <= SPATIAL_REUSE_COUNT; i += 1u) {
-        const Candidate cur = next;
-        next = prepare(i + 1u);
-        if (!cur.valid) continue;
-        const vec2 offset = cur.offset;
-        const float sample_depth = cur.sample_depth;
+    Gather ahead[HK_SPATIAL_GATHER_AHEAD + 1];
+#pragma unroll
+    for (int k = 0; k <= HK_SPATIAL_GATHER_AHEAD; ++k) ahead[k] = gather_next();
+    while (ahead[0].valid) {
+        const Gather cur = ahead[0];
+#pragma unroll
+        for (int k = 0; k < HK_SPATIAL_GATHER_AHEAD; ++k) ahead[k] = ahead[k + 1];
+        ahead[HK_SPATIAL_GATHER_AHEAD] = gather_next();
         PackedQuarters packed;
-        packed.q0 = cur.q0; packed.q1 = cur.q1; packed.q2 = cur.q2; packed.q3 = cur.q3;
+        packed.q0 = cur.q0; packed.q1 = cur.q1; packed.q2 = cur.q2; packed.q3 = s_q3[cur.cell];
         q = unpack_reservoir(packed);
         vec3 sample_direction = normalize(xyz(q.s.sample_position) - xyz(s.visible_position));
         if (dot(sample_direction, s.visible_normal) < 0.0f) continue;
-
-        // screen-space depth march towards the neighbour (light.wgsl:1608-1628), every tap out of the staged depth tile
-        const uint32_t tap_count = T.tap_count[i];
-        bool occluded = false;
-        vec2 unit = normalize(offset);
-        for (uint32_t j = 1u; j <= tap_count; j += 1u) {
-            float tap_dist = T.tap_dist[i][j - 1u];
-#if HK_SPATIAL_FAST_DIV
-            const vec2 tap_offset = tap_dist * unit;
-            const float qx = tap_offset.x * P.inv_rw, qy = tap_offset.y * P.inv_rh;
-            vec2 tap_uv = uv + v2(fmaf(fmaf(-qx, size_f.x, tap_offset.x), P.inv_rw, qx), fmaf(fmaf(-qy, size_f.y, tap_offset.y), P.inv_rh, qy));
-#else
-            vec2 tap_uv = uv + (tap_dist * unit) / size_f;
-#endif
-            int tx = f32_to_i32(tap_uv.x * (float)P.band.W), ty = f32_to_i32(tap_uv.y * (float)P.band.H);
-            float tap_depth = 0.0f;  // out-of-bounds textureLoad -> 0
-            if (tx >= 0 && tx < P.band.W && ty >= 0 && ty < P.band.H) {
-                // a tap lies between the pixel and its neighbour, hence inside the tile; a float coordinate that rounds one pixel
-                // out of it (never observed) falls back to the plane
-                const int cxl = tx - tx0, cyl = ty - ty0;
-                tap_depth = ((unsigned)cxl < (unsigned)BW && (unsigned)cyl < (unsigned)BH) ? s_depth[cyl * BW + cxl] : P.planes.pos_depth[band_index(P.band, tx, ty)].w;
-            }
-            float ref_depth = mixf(depth, sample_depth, T.tap_ratio[i][j - 1u]);
-            if (tap_depth > ref_depth + 0.00001f) { occluded = true; break; }
-        }
-        if (occluded) continue;
 
         float jacobian = (q.s.sample_position.w > 0.5f) ? compute_jacobian(q.s, s) : 1.0f;
         if (EMISSIVE_LIT) {
@@ -384,7 +448,7 @@ using namespace hkd;
 static inline bool no_texture(const KParams& P) { return HK_NO_TEXTURE_VARIANT && P.scene.texture_count == 0u; }
 
 template <bool EMISSIVE_LIT, bool TEX>
-static void launch_tiled(const KParams& P, const TileMap& depth_map, const TileMap& q3_map, cudaStream_t st) {
+static void launch_tiled(const KParams& P, const TileMap& depth_map, const TileMap& q3_map, const SpatialTable& table, cudaStream_t st) {
     const size_t smem = SpatialTile<EMISSIVE_LIT>::SMEM_BYTES;
     static bool configured[64] = {};     // per instantiation AND per device: the attribute belongs to the function on one device
     int dev = 0;
@@ -392,16 +456,17 @@ static void launch_tiled(const KParams& P, const TileMap& depth_map, const TileM
     if (!configured[dev & 63]) { cudaFuncSetAttribute(kc_spatial<EMISSIVE_LIT, TEX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); configured[dev & 63] = true; }
     const int rows = P.row_hi - P.row_lo, cols = P.col_hi - P.col_lo;
     const dim3 g((unsigned)((cols + POOL_TILE_W - 1) / POOL_TILE_W), (unsigned)((rows + POOL_TILE_H - 1) / POOL_TILE_H), 1u);
-    kc_spatial<EMISSIVE_LIT, TEX><<<g, POOL_THREADS, smem, st>>>(P, depth_map, q3_map);
+    kc_spatial<EMISSIVE_LIT, TEX><<<g, POOL_THREADS, smem, st>>>(P, depth_map, q3_map, table);
 }
 
 // `depth_map` / `q3_map`: TMA descriptors of the depth plane and of quarter 3 of the temporal reservoir this launch reuses, boxed for
-// this variant's radius (context.cu); nullptr (or an upscale ratio above 1) selects the gather-from-global form.
-void hk_launch_spatial(const KParams& P, bool emissive, const TileMap* depth_map, const TileMap* q3_map, cudaStream_t st) {
+// this variant's radius (context.cu); nullptr (or an upscale ratio above 1) selects the gather-from-global form.  `table`: host copy
+// of this pipeline's P.spatial_tables entry, which the tiled form takes as a kernel parameter.
+void hk_launch_spatial(const KParams& P, bool emissive, const TileMap* depth_map, const TileMap* q3_map, const SpatialTable& table, cudaStream_t st) {
     if (P.row_hi <= P.row_lo || P.col_hi <= P.col_lo) return;
     if (depth_map && q3_map && P.ratio1) {
-        if (no_texture(P)) { if (emissive) launch_tiled<true, false>(P, *depth_map, *q3_map, st); else launch_tiled<false, false>(P, *depth_map, *q3_map, st); }
-        else { if (emissive) launch_tiled<true, true>(P, *depth_map, *q3_map, st); else launch_tiled<false, true>(P, *depth_map, *q3_map, st); }
+        if (no_texture(P)) { if (emissive) launch_tiled<true, false>(P, *depth_map, *q3_map, table, st); else launch_tiled<false, false>(P, *depth_map, *q3_map, table, st); }
+        else { if (emissive) launch_tiled<true, true>(P, *depth_map, *q3_map, table, st); else launch_tiled<false, true>(P, *depth_map, *q3_map, table, st); }
         return;
     }
     if (no_texture(P)) {
