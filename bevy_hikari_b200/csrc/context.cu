@@ -22,7 +22,7 @@
 #include "wide_build.h"
 
 #ifndef HK_POOLED_INDIRECT
-#define HK_POOLED_INDIRECT 0     // default of hk_set_tuning(HK_TUNE_POOLED_INDIRECT): 0 = per-pixel k_indirect, 1 = kc_indirect (ray pool).
+#define HK_POOLED_INDIRECT 0     // default of hk_set_tuning(HK_TUNE_POOLED_INDIRECT): 0 = per-pixel k_indirect_path + k_indirect_restir, 1 = kc_indirect (ray pool).
 #endif                            // Same values either way; the per-pixel form is the default.
 
 #ifndef HK_WIDE_TRAVERSAL_DEFAULT
@@ -1071,7 +1071,7 @@ static int run_light(hk_context* ctx, KParams& P) {  // LightNode::run order, li
       hk_launch_scatter_resolve(P, 1, ctx->stream); ctx->launches += 1; }
     if (f.emissive_spatial_reuse) { rows(ctx, P, GHOST_SPATIAL); KernelTimer t(ctx, HK_K_EMISSIVE_SPATIAL); launch_spatial(ctx, P, true); }
     rows(ctx, P, GHOST_TEMPORAL + ctx->motion_margin);
-    { KernelTimer t(ctx, HK_K_INDIRECT);
+    { KernelTimer t(ctx, HK_K_INDIRECT);   // the per-pixel form's two kernels (path, then ReSTIR tail) count as one launch, as the pooled one
       if (ctx->pooled_indirect) hk_launch_indirect_pool(P, f.indirect_bounces >= 2, ctx->count_rays, ctx->stream);
       else hk_launch_indirect(P, f.indirect_bounces >= 2, ctx->count_rays, wide_light(ctx), ctx->stream);
       hk_launch_scatter_resolve(P, 2, ctx->stream); ctx->launches += 1; }

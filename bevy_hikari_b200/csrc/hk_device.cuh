@@ -941,6 +941,9 @@ constexpr int TILE_W = 16, TILE_H = 2 * HK_CTA_WARPS, CTA_THREADS = 32 * HK_CTA_
                              // 8 CTAs/SM (64 registers) 2.87 / 27.2 / 15.7, 12 (40 registers, spills) 2.95 / 26.0 / 15.3, 16 (32 registers)
                              // 3.31 / 25.4 / 15.6.  8 is chosen for the benchmark workload; deeper scenes want more warps (DESIGN.md 6b)
 #endif
+#ifndef HK_MINB_INDIRECT_RESTIR
+#define HK_MINB_INDIRECT_RESTIR 5   // k_indirect_restir, the ReSTIR-GI tail of the indirect pass: 8 CTAs/SM (64 registers) spill 120 B, 5 take 94 without spills
+#endif
 #ifndef HK_MINB_DIRECT
 #define HK_MINB_DIRECT 8
 #endif

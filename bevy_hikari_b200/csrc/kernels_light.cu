@@ -334,47 +334,55 @@ __global__ void __launch_bounds__(CTA_THREADS, WIDE ? HK_MINB_DIRECT_WIDE : HK_M
 }
 
 // ----------------------------------------------------------------------------- P3: indirect_lit_ambient
-// light.wgsl:1263-1498.  One kernel covers both the single-bounce and the MULTIPLE_BOUNCES variants: the reference's
-// single-bounce body is the loop body for n == 0 without the luminance clamp, so MULTI only switches those two bits.
+// light.wgsl:1263-1498 as two kernels over the same pixels.  k_indirect_path traces the path of every surface pixel and keeps
+// alive only what the walk needs; k_indirect_restir then runs the temporal ReSTIR-GI tail with coherent warps and no ray.
+// Between them the path's four results travel at full f32 precision through the scatter_value planes: those carry a reservoir
+// only from a validation write of k_direct to the k_scatter_resolve of the same pass, which has run before this pass starts.
+struct PathResult { vec4 radiance, sample_position; vec3 sample_normal; float pdf; };
+// the first bounce's hit is stored as soon as it is known, so that it is not carried through the later bounces
+__device__ __forceinline__ void store_path_sample(const KParams& P, size_t idx, vec4 sample_position, vec3 sample_normal, float pdf) {
+    P.planes.scatter_value.q[1][idx] = make_uint4(__float_as_uint(sample_position.x), __float_as_uint(sample_position.y),
+                                                  __float_as_uint(sample_position.z), __float_as_uint(sample_position.w));
+    P.planes.scatter_value.q[2][idx] = make_uint4(__float_as_uint(sample_normal.x), __float_as_uint(sample_normal.y),
+                                                  __float_as_uint(sample_normal.z), __float_as_uint(pdf));
+}
+__device__ __forceinline__ void store_path_radiance(const KParams& P, size_t idx, vec4 radiance) {
+    P.planes.scatter_value.q[0][idx] = make_uint4(__float_as_uint(radiance.x), __float_as_uint(radiance.y),
+                                                  __float_as_uint(radiance.z), __float_as_uint(radiance.w));
+}
+__device__ __forceinline__ PathResult load_path(const KParams& P, size_t idx) {
+    const uint4 a = P.planes.scatter_value.q[0][idx], b = P.planes.scatter_value.q[1][idx], c = P.planes.scatter_value.q[2][idx];
+    PathResult r;
+    r.radiance = v4(__uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z), __uint_as_float(a.w));
+    r.sample_position = v4(__uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z), __uint_as_float(b.w));
+    r.sample_normal = v3(__uint_as_float(c.x), __uint_as_float(c.y), __uint_as_float(c.z));
+    r.pdf = __uint_as_float(c.w);
+    return r;
+}
+__device__ __forceinline__ bool indirect_background(const KParams& P, float depth) {
+    return P.in.frame.indirect_bounces == 0u || depth < F32_EPSILON;
+}
+
+// The bounce loop.  One kernel covers both the single-bounce and the MULTIPLE_BOUNCES variants: the reference's single-bounce
+// body is the loop body for n == 0 without the luminance clamp, so MULTI only switches those two bits.
 template <bool MULTI, bool COUNT, bool TEX = true, bool WIDE = false>
-__global__ void __launch_bounds__(CTA_THREADS, WIDE ? HK_MINB_INDIRECT_WIDE : HK_MINB_INDIRECT) k_indirect(const __grid_constant__ KParams P) {
+__global__ void __launch_bounds__(CTA_THREADS, WIDE ? HK_MINB_INDIRECT_WIDE : HK_MINB_INDIRECT) k_indirect_path(const __grid_constant__ KParams P) {
     int x, y;
     tile_pixel(x, y, P);
     const bool active = tile_active(P, x, y);
     uint32_t n_tlas = 0, n_blas = 0;
     if (active) {
-        const DeviceScene sc = scene_variant<TEX>(P.scene);
-        const hk_frame_uniform& frame = P.in.frame;
         const size_t idx = render_index(P.band, x, y);
         const size_t gidx = light_gbuffer_index(P, x, y, idx);
-        const PassBuffers B = bind(P, 2);
         const float4 pd = P.planes.pos_depth[gidx];
-        const float depth = pd.w;
-        if (frame.indirect_bounces == 0u || depth < F32_EPSILON) {
-            PackedQuarters q = pack_reservoir(zero_reservoir());
-            store_quarters(B.reservoir, idx, q);
-            store_quarters(B.spatial_reservoir, idx, q);
-            scatter_claim(P, idx, x, y, SCATTER_BACKGROUND);
-            P.planes.variance[2][idx] = 0.0f;
-            P.planes.render[2][idx] = make_uint2(0u, 0u);
-        } else {
+        if (!indirect_background(P, pd.w)) {
+            const DeviceScene sc = scene_variant<TEX>(P.scene);
+            const hk_frame_uniform& frame = P.in.frame;
             const ShadeEnv env = make_env(P);
-            const vec3 position = f4xyz(pd);
-            const vec3 normal = normalize(xyz(unpack4x8snorm(P.planes.normal[gidx])));  // normalised here (light.wgsl:1289)
-            const float2 imf = P.planes.instance_material[gidx];
-            const uint32_t instance_id = f32_to_u32(imf.x), material_id = f32_to_u32(imf.y);
-            const float4 vu = P.planes.velocity_uv[gidx];
-
-            Sample s = zero_sample();
-            s.random = noise_random(P, x, y);
-            s.visible_position = v4(position, depth);
-            s.visible_normal = normal;
-            s.visible_instance = instance_id;
-
-            float pdf = 0.0f;
+            vec4 radiance = v4(0.0f);
             // bounce state: the vertex we are leaving
-            vec3 b_position = position, b_normal = normal;
-            vec4 b_random = s.random;
+            vec3 b_position = f4xyz(pd), b_normal = normalize(xyz(unpack4x8snorm(P.planes.normal[gidx])));  // normalised here (light.wgsl:1289)
+            vec4 b_random = noise_random(P, x, y);
             vec3 color_transport = v3(1.0f);
             const uint32_t bounces = MULTI ? frame.indirect_bounces : 1u;
             for (uint32_t n = 0u; n < bounces && (color_transport.x > 0.01f || color_transport.y > 0.01f || color_transport.z > 0.01f); n += 1u) {
@@ -386,11 +394,7 @@ __global__ void __launch_bounds__(CTA_THREADS, WIDE ? HK_MINB_INDIRECT_WIDE : HK
                 if (COUNT) n_tlas += 1u;
                 Hit hit = trace_top<WIDE>(sc, ray, F32_MAX, 0.0f, DONT_EXCLUDE);
                 HitInfo info = hit_info(sc, ray, hit);
-                if (n == 0u) {
-                    s.sample_position = info.position;
-                    s.sample_normal = info.normal;
-                    pdf = rand_sample.w;
-                }
+                if (n == 0u) store_path_sample(P, idx, info.position, info.normal, rand_sample.w);
                 const vec3 h_position = xyz(info.position), h_normal = info.normal;
                 if (hit.instance_index != U32_MAX) {
                     vec3 out_radiance = v3(0.0f);
@@ -414,9 +418,9 @@ __global__ void __launch_bounds__(CTA_THREADS, WIDE ? HK_MINB_INDIRECT_WIDE : HK
                             float out_luminance = luminance(out_radiance);
                             if (out_luminance > frame.max_indirect_luminance)
                                 out_radiance = out_radiance * frame.max_indirect_luminance / out_luminance;
-                            s.radiance = s.radiance + v4(color_transport * out_radiance, 1.0f);
+                            radiance = radiance + v4(color_transport * out_radiance, 1.0f);
                         } else {
-                            s.radiance = s.radiance + v4(out_radiance, 1.0f);
+                            radiance = radiance + v4(out_radiance, 1.0f);
                         }
                     }
                     if (MULTI) {
@@ -427,42 +431,84 @@ __global__ void __launch_bounds__(CTA_THREADS, WIDE ? HK_MINB_INDIRECT_WIDE : HK
                     }
                 } else {
                     vec3 out_radiance = xyz(input_radiance(sc, env, ray.direction, info, false, DONT_SAMPLE_EMISSIVE, true));
-                    s.radiance = MULTI ? s.radiance + v4(color_transport * out_radiance, 0.0f) : s.radiance + v4(out_radiance, 0.0f);
+                    radiance = MULTI ? radiance + v4(color_transport * out_radiance, 0.0f) : radiance + v4(out_radiance, 0.0f);
                     break;
                 }
             }
-
-            // ReSTIR: temporal
-            const vec2 previous_uv = jittered_deferred_uv(P, pixel_uv(P, x, y), 0.25f) - v2(vu.x, vu.y);
-            size_t pidx = 0;
-            Reservoir r = zero_reservoir();
-            if (previous_pixel(P, previous_uv, false, pidx)) r = unpack_reservoir(load_quarters(B.previous_reservoir, pidx));
-            if (!check_previous_reservoir(r, s)) {
-                size_t sidx;
-                if (previous_pixel(P, previous_uv, true, sidx)) scatter_claim(P, sidx, x, y, SCATTER_MISS);
-            }
-            Surface surface = retreive_surface(sc, material_id, v2(vu.z, vu.w));
-            vec3 view_direction = calculate_view(env, position);
-            vec3 sample_radiance = shading(env, view_direction, s.visible_normal,
-                                           normalize(xyz(s.sample_position) - xyz(s.visible_position)), surface, s.radiance);
-            float w_new = (pdf > 0.0f) ? luminance(sample_radiance) / pdf : 0.0f;
-            temporal_restir(r, s, w_new, frame.max_temporal_reuse_count);
-
-            vec3 out_radiance = shading(env, view_direction, r.s.visible_normal,
-                                        normalize(xyz(r.s.sample_position) - xyz(r.s.visible_position)), surface, r.s.radiance);
-            float total_lum = r.count * luminance(out_radiance);
-            r.w = (total_lum > 0.0f) ? r.w_sum / total_lum : 0.0f;
-            r.s.visible_position = s.visible_position;
-            r.s.visible_normal = s.visible_normal;
-            r.lifetime += 1.0f;
-            P.planes.variance[2][idx] = variance_of(r);
-            if (frame.temporal_reuse > 0u) store_quarters(B.reservoir, idx, pack_reservoir(r));
-            uvec2 o = pack_rgba16f(v4(out_radiance * r.w, 1.0f));
-            P.planes.render[2][idx] = make_uint2(o.x, o.y);
+            store_path_radiance(P, idx, radiance);
         }
     }
     if (!band_owned(P.band, x, y)) { n_tlas = 0; n_blas = 0; }   // ghost pixels are redundant work: not counted
     flush_counters<COUNT>(P, 0u, n_tlas, n_blas);
+}
+
+// The temporal ReSTIR-GI tail over k_indirect_path's results: reservoir reuse, shading, variance and the scatter claims.
+template <bool TEX = true>
+__global__ void __launch_bounds__(CTA_THREADS, HK_MINB_INDIRECT_RESTIR) k_indirect_restir(const __grid_constant__ KParams P) {
+    int x, y;
+    tile_pixel(x, y, P);
+    if (!tile_active(P, x, y)) return;
+    const DeviceScene sc = scene_variant<TEX>(P.scene);
+    const hk_frame_uniform& frame = P.in.frame;
+    const size_t idx = render_index(P.band, x, y);
+    const size_t gidx = light_gbuffer_index(P, x, y, idx);
+    const PassBuffers B = bind(P, 2);
+    const float4 pd = P.planes.pos_depth[gidx];
+    const float depth = pd.w;
+    if (indirect_background(P, depth)) {
+        PackedQuarters q = pack_reservoir(zero_reservoir());
+        store_quarters(B.reservoir, idx, q);
+        store_quarters(B.spatial_reservoir, idx, q);
+        scatter_claim(P, idx, x, y, SCATTER_BACKGROUND);
+        P.planes.variance[2][idx] = 0.0f;
+        P.planes.render[2][idx] = make_uint2(0u, 0u);
+    } else {
+        const ShadeEnv env = make_env(P);
+        const vec3 position = f4xyz(pd);
+        const vec3 normal = normalize(xyz(unpack4x8snorm(P.planes.normal[gidx])));  // normalised here (light.wgsl:1289)
+        const float2 imf = P.planes.instance_material[gidx];
+        const uint32_t instance_id = f32_to_u32(imf.x), material_id = f32_to_u32(imf.y);
+        const float4 vu = P.planes.velocity_uv[gidx];
+
+        const PathResult path = load_path(P, idx);
+        Sample s = zero_sample();
+        s.random = noise_random(P, x, y);
+        s.visible_position = v4(position, depth);
+        s.visible_normal = normal;
+        s.visible_instance = instance_id;
+        s.radiance = path.radiance;
+        s.sample_position = path.sample_position;
+        s.sample_normal = path.sample_normal;
+        const float pdf = path.pdf;
+
+        // ReSTIR: temporal
+        const vec2 previous_uv = jittered_deferred_uv(P, pixel_uv(P, x, y), 0.25f) - v2(vu.x, vu.y);
+        size_t pidx = 0;
+        Reservoir r = zero_reservoir();
+        if (previous_pixel(P, previous_uv, false, pidx)) r = unpack_reservoir(load_quarters(B.previous_reservoir, pidx));
+        if (!check_previous_reservoir(r, s)) {
+            size_t sidx;
+            if (previous_pixel(P, previous_uv, true, sidx)) scatter_claim(P, sidx, x, y, SCATTER_MISS);
+        }
+        Surface surface = retreive_surface(sc, material_id, v2(vu.z, vu.w));
+        vec3 view_direction = calculate_view(env, position);
+        vec3 sample_radiance = shading(env, view_direction, s.visible_normal,
+                                       normalize(xyz(s.sample_position) - xyz(s.visible_position)), surface, s.radiance);
+        float w_new = (pdf > 0.0f) ? luminance(sample_radiance) / pdf : 0.0f;
+        temporal_restir(r, s, w_new, frame.max_temporal_reuse_count);
+
+        vec3 out_radiance = shading(env, view_direction, r.s.visible_normal,
+                                    normalize(xyz(r.s.sample_position) - xyz(r.s.visible_position)), surface, r.s.radiance);
+        float total_lum = r.count * luminance(out_radiance);
+        r.w = (total_lum > 0.0f) ? r.w_sum / total_lum : 0.0f;
+        r.s.visible_position = s.visible_position;
+        r.s.visible_normal = s.visible_normal;
+        r.lifetime += 1.0f;
+        P.planes.variance[2][idx] = variance_of(r);
+        if (frame.temporal_reuse > 0u) store_quarters(B.reservoir, idx, pack_reservoir(r));
+        uvec2 o = pack_rgba16f(v4(out_radiance * r.w, 1.0f));
+        P.planes.render[2][idx] = make_uint2(o.x, o.y);
+    }
 }
 
 // depth plane <- pos_depth.w (after hk_upload_state of the position plane)
@@ -579,12 +625,14 @@ template <bool WIDE>
 static void launch_indirect(const KParams& P, bool multi, bool count, cudaStream_t st) {
     dim3 g = grid_for(P);
     if (!count && no_texture(P)) {
-        if (multi) k_indirect<true, false, false, WIDE><<<g, CTA_THREADS, 0, st>>>(P);
-        else k_indirect<false, false, false, WIDE><<<g, CTA_THREADS, 0, st>>>(P);
+        if (multi) k_indirect_path<true, false, false, WIDE><<<g, CTA_THREADS, 0, st>>>(P);
+        else k_indirect_path<false, false, false, WIDE><<<g, CTA_THREADS, 0, st>>>(P);
+        k_indirect_restir<false><<<g, CTA_THREADS, 0, st>>>(P);
         return;
     }
-    if (multi) { if (count) k_indirect<true, true, true, WIDE><<<g, CTA_THREADS, 0, st>>>(P); else k_indirect<true, false, true, WIDE><<<g, CTA_THREADS, 0, st>>>(P); }
-    else { if (count) k_indirect<false, true, true, WIDE><<<g, CTA_THREADS, 0, st>>>(P); else k_indirect<false, false, true, WIDE><<<g, CTA_THREADS, 0, st>>>(P); }
+    if (multi) { if (count) k_indirect_path<true, true, true, WIDE><<<g, CTA_THREADS, 0, st>>>(P); else k_indirect_path<true, false, true, WIDE><<<g, CTA_THREADS, 0, st>>>(P); }
+    else { if (count) k_indirect_path<false, true, true, WIDE><<<g, CTA_THREADS, 0, st>>>(P); else k_indirect_path<false, false, true, WIDE><<<g, CTA_THREADS, 0, st>>>(P); }
+    k_indirect_restir<true><<<g, CTA_THREADS, 0, st>>>(P);
 }
 void hk_launch_indirect(const KParams& P, bool multi, bool count, bool wide, cudaStream_t st) {
     if (P.row_hi <= P.row_lo || P.col_hi <= P.col_lo) return;

@@ -298,7 +298,7 @@ int hk_set_profiling_kernel(hk_context* ctx, int kernel);
 /* Implementation choices.  Keys 1-3 do not change a single output value (both forms are held to the same parity suite); key 4 is
  * the image-exact traversal mode, which keeps every image but not every record (below).
  * HK_TUNE_POOLED_INDIRECT: 1 = the indirect pass runs as kc_indirect (per-CTA shared-memory ray pool, dynamic fetch, TMA-staged scene
- * records, kernels_pool.cu), 0 = as the per-pixel k_indirect (default, DESIGN.md 4).
+ * records, kernels_pool.cu), 0 = per pixel, k_indirect_path + k_indirect_restir (default, DESIGN.md 4).
  * HK_TUNE_TILED_SPATIAL: 1 (default) = spatial_reuse runs as kc_spatial (neighbourhood depth + reservoir-quarter tiles staged in shared
  * memory by TMA, kernels_spatial.cu) whenever the upscale ratio is 1, 0 = as k_spatial (gathers from global memory).
  * HK_TUNE_TILED_DENOISE: 1 (default) = the a-trous levels run as kc_denoise (the nine taps' planes staged by TMA, kernels_post.cu) at
