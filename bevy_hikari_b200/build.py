@@ -41,7 +41,7 @@ CXX = os.environ.get("HK_CXX", "/usr/bin/g++")
 CU = ["csrc/context.cu", "csrc/kernels_light.cu", "csrc/kernels_pool.cu", "csrc/kernels_spatial.cu", "csrc/kernels_post.cu", "csrc/kernels_upscale.cu", "csrc/kernels_scene.cu"]
 CPP_HOST = ["host/hikari.cpp", "host/hikari_capi.cpp", "host/gltf_ingest.cpp"]                     # -> libhikari_host.so
 CPP_PLUGIN = ["host/hikari_plugin.cpp", "host/hikari_plugin_capi.cpp"]     # -> libhikari_b200.so (they call hk_*)
-HEADERS = ["csrc/hk_device.cuh", "csrc/hk_pool.cuh", "csrc/hk_wide.cuh", "csrc/wide_build.h", "csrc/hk_tile.cuh", "csrc/hk_kernels.h", "host/hikari.hpp", "host/hikari_settings_convert.hpp",
+HEADERS = ["csrc/hk_device.cuh", "csrc/hk_pool.cuh", "csrc/hk_wide.cuh", "csrc/wide_build.h", "csrc/hk_tile.cuh", "csrc/hk_spatial_taps.cuh", "csrc/hk_kernels.h", "host/hikari.hpp", "host/hikari_settings_convert.hpp",
            "../include/hk_math.h", "../include/hk_layout.h", "../include/hikari_b200.h", "../include/hikari_host.h"]
 
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-fmad=false",
@@ -121,6 +121,37 @@ def build(force=False, verbose=False, ptxas_info=False, out=None):
     if verbose or ptxas_info:
         print("\n".join(l for l in logs if l.strip()))
     return lib
+
+
+PROBE_SRC = os.path.join(ROOT, "tests", "cuda", "math_probe.cu")
+PROBE_LIBS = {"exact": os.path.join(OBJ, "libhk_math_probe_exact.so"), "fast": os.path.join(OBJ, "libhk_math_probe_fast.so")}
+
+
+def probe_flags(flavor):
+    """nvcc flags of the math probe: those of every unit that traces rays ("exact") or those of FAST_TUS ("fast"), derived from
+    NVCC_FLAGS / FAST_FLAGS exactly as build() derives them."""
+    fast = flavor == "fast"
+    return [f for f in NVCC_FLAGS if not (fast and f == "-fmad=false")] + (FAST_FLAGS if fast else [])
+
+
+def build_math_probe(force=False):
+    """Test infrastructure: tests/cuda/math_probe.cu (the primitives of include/hk_math.h and the spatial-reuse pixel helpers run
+    on the device) as two shared libraries, one per flavour; tests/test_gpu_device_math.py compares them with the oracle."""
+    os.makedirs(OBJ, exist_ok=True)
+    sources = [PROBE_SRC] + [os.path.join(HERE, h) for h in HEADERS]
+    jobs = []
+    for flavor, lib in PROBE_LIBS.items():
+        flags = probe_flags(flavor)
+        stamp = lib + ".flags"
+        stale = not os.path.exists(stamp) or open(stamp).read() != " ".join(flags)
+        if force or stale or _newer(lib, sources):
+            jobs.append(([NVCC] + flags + ["-shared", "-cudart", "static", "-o", lib, PROBE_SRC], stamp, flags))
+    if jobs:
+        with ThreadPoolExecutor(max_workers=len(jobs)) as ex:
+            list(ex.map(lambda j: _run(j[0]), jobs))
+        for _, stamp, flags in jobs:
+            open(stamp, "w").write(" ".join(flags))
+    return dict(PROBE_LIBS)
 
 
 if __name__ == "__main__":

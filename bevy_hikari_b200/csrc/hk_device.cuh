@@ -254,7 +254,7 @@ static __device__ HK_INL_PACK PackedQuarters pack_reservoir(const Reservoir& r) 
                       __float_as_uint(r.s.visible_position.z), __float_as_uint(r.s.visible_position.w));
     p.q2 = make_uint4(__float_as_uint(r.s.sample_position.x), __float_as_uint(r.s.sample_position.y),
                       __float_as_uint(r.s.sample_position.z), __float_as_uint((float)r.s.visible_instance));
-    p.q3.x = pack4x8snorm(v4(r.s.visible_normal, r.lifetime / 127.0f - 1.0f));
+    p.q3.x = pack4x8snorm(v4(r.s.visible_normal, add_rn(div_rn(r.lifetime, 127.0f), -1.0f)));   // IEEE in a tolerance unit too
     p.q3.y = pack4x8snorm(v4(r.s.sample_normal, r.s.sample_position.w));
     p.q3.z = pack2x16float(r.count, r.w);
     p.q3.w = pack2x16float(r.w_sum, r.w2_sum);

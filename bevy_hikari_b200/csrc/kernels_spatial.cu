@@ -8,14 +8,12 @@
 #ifndef HK_NO_TEXTURE_VARIANT
 #define HK_NO_TEXTURE_VARIANT 1
 #endif
-// Requesting a neighbour's reservoir together with its depth, and dividing by the frame size with a host-computed reciprocal (exact
-// whenever the quotient is normal); =0 restores the two-step load / the division for A/B runs.
+// Requesting a neighbour's reservoir together with its depth (=0 restores the two-step load for A/B runs).  The depth march's
+// division by the frame size, HK_SPATIAL_FAST_DIV, is a switch of hk_spatial_taps.cuh.
 #ifndef HK_SPATIAL_EAGER_LOAD
 #define HK_SPATIAL_EAGER_LOAD 1
 #endif
-#ifndef HK_SPATIAL_FAST_DIV
-#define HK_SPATIAL_FAST_DIV 1
-#endif
+#include "hk_spatial_taps.cuh"
 
 // CTAs of 256 threads per SM of the tiled kernel: 74 KB of shared memory each for the indirect pipeline (at most 3 fit), 32 KB for the
 // emissive one.  2 CTAs/SM = 127 registers without spills rather than 3 CTAs/SM = 80 registers with spills (slower on the H100)
@@ -102,13 +100,11 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_SPATIAL) k_spatial(const 
     const vec2 size_f = v2((float)P.band.RW, (float)P.band.RH);
     const SpatialTable& T = P.spatial_tables[EMISSIVE_LIT ? 1 : 0];
     const float rotation = sum4(s.random);
+    const vec2 march_uv = spatial_pixel_uv(x, y, size_f.x, size_f.y);     // = uv, rounded the oracle's way in the tolerance build too
     for (uint32_t i = 1u; i <= SPATIAL_REUSE_COUNT; i += 1u) {
-        float ang = TAU * fract(T.phase[i] + rotation + P.random_frame);
-        const float rad = T.radius[i];
-        float sn, cs;
-        sincos_(ang, &sn, &cs);
-        vec2 offset = rad * v2(cs, sn);
-        int sx = f32_to_i32(offset.x + (float)x), sy = f32_to_i32(offset.y + (float)y);
+        const vec2 offset = spatial_offset(T.phase[i], T.radius[i], rotation, P.random_frame);
+        int sx, sy;
+        spatial_neighbour_pixel(offset, x, y, sx, sy);
         // light.wgsl:1577-1580 tests sample_uv = (coords + 0.5) / size against [0, 1].  For integer coords and size < 2^22
         // the correctly rounded quotient is < 0 iff coords < 0 and > 1 iff coords >= size ((size - 0.5) / size < 1 and
         // (size + 0.5) / size >= 1 + 2^-23 survive rounding), so the two IEEE divisions per neighbour are not needed.
@@ -140,20 +136,9 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_SPATIAL) k_spatial(const 
         // screen-space depth march towards the neighbour (light.wgsl:1608-1628)
         const uint32_t tap_count = T.tap_count[i];
         bool occluded = false;
-        vec2 unit = normalize(offset);
+        const vec2 unit = spatial_march_unit(offset);
         for (uint32_t j = 1u; j <= tap_count; j += 1u) {
-            float tap_dist = T.tap_dist[i][j - 1u];
-#if HK_SPATIAL_FAST_DIV
-            // Default since round 2 (-DHK_SPATIAL_FAST_DIV=0 restores the IEEE division): x / C for the frame constant C as q = x * y, r = fma(-q, C, x), fma(r, y, q)
-            // with y = RN(1 / C) from the host — the correctly rounded quotient whenever it is a normal number
-            // (tools/check_runtime_division.cpp: all 2^32 inputs for the benchmark extents); a subnormal quotient is absorbed
-            // by the addition to uv >= 0.5 / size.
-            const vec2 tap_offset = tap_dist * unit;
-            const float qx = tap_offset.x * P.inv_rw, qy = tap_offset.y * P.inv_rh;
-            vec2 tap_uv = uv + v2(fmaf(fmaf(-qx, size_f.x, tap_offset.x), P.inv_rw, qx), fmaf(fmaf(-qy, size_f.y, tap_offset.y), P.inv_rh, qy));
-#else
-            vec2 tap_uv = uv + (tap_dist * unit) / size_f;
-#endif
+            vec2 tap_uv = spatial_tap_uv(march_uv, unit, T.tap_dist[i][j - 1u], size_f.x, size_f.y, P.inv_rw, P.inv_rh);
             vec2 tap_deferred_uv = jittered_deferred_uv(P, tap_uv, 0.25f);
             int tx = f32_to_i32(tap_deferred_uv.x * (float)P.band.W), ty = f32_to_i32(tap_deferred_uv.y * (float)P.band.H);
             float tap_depth = 0.0f;  // out-of-bounds textureLoad -> 0
@@ -193,15 +178,7 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_SPATIAL) k_spatial(const 
 // Frame pixel (tx, ty) of tap j (1-based) of neighbour i's screen-space depth march (light.wgsl:1608-1628) at upscale ratio 1
 __device__ __forceinline__ void march_tap(const KParams& P, const SpatialTable& T, uint32_t i, uint32_t j, vec2 uv, vec2 size_f, vec2 unit,
                                           int& tx, int& ty) {
-    float tap_dist = T.tap_dist[i][j - 1u];
-#if HK_SPATIAL_FAST_DIV
-    const vec2 tap_offset = tap_dist * unit;
-    const float qx = tap_offset.x * P.inv_rw, qy = tap_offset.y * P.inv_rh;
-    vec2 tap_uv = uv + v2(fmaf(fmaf(-qx, size_f.x, tap_offset.x), P.inv_rw, qx), fmaf(fmaf(-qy, size_f.y, tap_offset.y), P.inv_rh, qy));
-#else
-    vec2 tap_uv = uv + (tap_dist * unit) / size_f;
-#endif
-    tx = f32_to_i32(tap_uv.x * (float)P.band.W); ty = f32_to_i32(tap_uv.y * (float)P.band.H);
+    spatial_tap_pixel(spatial_tap_uv(uv, unit, T.tap_dist[i][j - 1u], size_f.x, size_f.y, P.inv_rw, P.inv_rh), P.band.W, P.band.H, tx, ty);
 }
 // The depth march of neighbour i with every tap read from the G-buffer instead of the staged tile: kc_spatial's fallback when a tap
 // lies in the frame but outside the tile (a tap lies between the pixel and its neighbour, hence inside it; a float coordinate that
@@ -329,6 +306,7 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
 
     const vec2 size_f = v2((float)P.band.RW, (float)P.band.RH);
     const float rotation = sum4(s.random);
+    const vec2 march_uv = spatial_pixel_uv(x, y, size_f.x, size_f.y);     // = uv, rounded the oracle's way in the tolerance build too
     mbar_wait(s_bar, 0u);                               // the tiles have landed
 
     // Stage A, shared memory only: every test that rejects a neighbour without its gathered quarters — bounds, depth ratio, count
@@ -338,12 +316,9 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
     uint32_t survivors = 0u;                            // bit i: neighbour i passed stage A
 #pragma unroll
     for (uint32_t i = 1u; i <= SPATIAL_REUSE_COUNT; i += 1u) {
-        float ang = TAU * fract(T.phase[i] + rotation + P.random_frame);
-        const float rad = T.radius[i];
-        float sn, cs;
-        sincos_(ang, &sn, &cs);
-        const vec2 offset = rad * v2(cs, sn);
-        int sx = f32_to_i32(offset.x + (float)x), sy = f32_to_i32(offset.y + (float)y);
+        const vec2 offset = spatial_offset(T.phase[i], T.radius[i], rotation, P.random_frame);
+        int sx, sy;
+        spatial_neighbour_pixel(offset, x, y, sx, sy);
         if (sx < 0 || sy < 0 || sx >= P.band.RW || sy >= P.band.RH) continue;      // see k_spatial
         const int tcell = (sy - ty0) * BW + (sx - tx0);
         const float sample_depth = s_depth[tcell];
@@ -361,11 +336,11 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
         // u32(radius / max(1, radius / 5)).
         const uint32_t tap_count = T.tap_count[i];
         bool occluded = false, from_plane = tap_count > 5u;
-        vec2 unit = normalize(offset);
+        const vec2 unit = spatial_march_unit(offset);
 #pragma unroll
         for (uint32_t j = 1u; j <= 5u; j += 1u) {
             int tx, ty;
-            march_tap(P, T, i, j, uv, size_f, unit, tx, ty);
+            march_tap(P, T, i, j, march_uv, size_f, unit, tx, ty);
             const bool in_frame = tx >= 0 && tx < P.band.W && ty >= 0 && ty < P.band.H;      // out-of-bounds textureLoad -> 0
             const int cxl = tx - tx0, cyl = ty - ty0;
             const bool in_tile = (unsigned)cxl < (unsigned)BW && (unsigned)cyl < (unsigned)BH;
@@ -375,7 +350,7 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
             from_plane |= live && in_frame && !in_tile;
             occluded |= live && tap_depth > mixf(depth, sample_depth, T.tap_ratio[i][j - 1u]) + 0.00001f;
         }
-        if (from_plane) occluded = march_occluded_from_plane(P, T, i, uv, size_f, unit, depth, sample_depth);
+        if (from_plane) occluded = march_occluded_from_plane(P, T, i, march_uv, size_f, unit, depth, sample_depth);
         if (occluded) continue;
         survivors |= 1u << i;
         s_cell[(i - 1u) * POOL_THREADS + threadIdx.x] = (uint16_t)tcell;

@@ -14,9 +14,14 @@
 //   * pack/unpack follow the WGSL spec formulas (floor(0.5 + s*clamp(x))) and RNE for f16.
 //
 // HK_FAST_MATH (device code of the product build's tolerance units only — kernels that trace no rays, see
-// bevy_hikari_b200/build.py): exp2_ is the hardware ex2.approx (2 ulp) instead of the polynomial, and the translation unit is
-// compiled with FMA contraction and approximate division / square root.  sincos_ stays the exact routine everywhere: the
-// spatial-reuse pass turns its result into integer pixel offsets, where an error of 1e-7 radians flips a neighbour now and then.
+// bevy_hikari_b200/build.py): exp2_ is the hardware ex2.approx (within 2.06 ulp on [-126, 128): 2.055 measured over every input on
+// an H100) instead of the polynomial, and the translation unit is
+// compiled with FMA contraction and approximate division / square root.  What ends in an integer stays exact there too:
+// sincos_ (the spatial-reuse pass turns its result into integer pixel offsets, where an error of 1e-7 radians flips a neighbour
+// now and then) and the snorm8 / unorm16 encodings write every product and sum as mul_rn / add_rn, which nvcc never contracts
+// into an FMA whatever -fmad says.  The neighbour and depth-march pixels of spatial reuse at upscale ratio 1 do the same
+// (csrc/hk_spatial_taps.cuh).
+// tests/test_gpu_device_math.py compares the device build of these primitives, exact and tolerance flavour, with the oracle's.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -50,12 +55,26 @@ constexpr uint32_t DONT_EXCLUDE = 0xFFFFFFFFu;      // light.wgsl:241
 constexpr uint32_t DONT_SAMPLE_EMISSIVE = 0x80000000u;  // light.wgsl:243
 
 // ---------------------------------------------------------------------------------------------- scalars
+// The host branches below exist only to mirror what the H100 computes (tests/test_gpu_device_math.py compares them bit for bit).
+// The device's arithmetic returns every NaN it produces as 0x7FFFFFFF, whatever the operands; x86 returns 0xFFC00000 or the
+// first operand's payload.  canon_nan gives the host the device's encoding where a primitive's result can be a NaN.
+HK_HD uint32_t f2u(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
+HK_HD float u2f(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
+HK_HD float canon_nan(float x) {
+#if defined(__CUDA_ARCH__)
+    return x;
+#else
+    return (x != x) ? u2f(0x7FFFFFFFu) : x;
+#endif
+}
+// min.f32 / max.f32: IEEE minNum / maxNum (a NaN operand yields the other operand), -0 below +0, two NaNs give 0x7FFFFFFF
 HK_HD float fmin_(float a, float b) {
 #if defined(__CUDA_ARCH__)
     return fminf(a, b);
 #else
     float m = (a < b) ? a : b;      // minss: returns b when unordered
-    return (b != b) ? a : m;        // IEEE minNum
+    if (a == b) m = u2f(f2u(a) | f2u(b));       // min(+0, -0) = -0 in either order
+    return (b != b) ? ((a != a) ? u2f(0x7FFFFFFFu) : a) : m;
 #endif
 }
 HK_HD float fmax_(float a, float b) {
@@ -63,18 +82,56 @@ HK_HD float fmax_(float a, float b) {
     return fmaxf(a, b);
 #else
     float m = (a > b) ? a : b;
-    return (b != b) ? a : m;
+    if (a == b) m = u2f(f2u(a) & f2u(b));       // max(+0, -0) = +0 in either order
+    return (b != b) ? ((a != a) ? u2f(0x7FFFFFFFu) : a) : m;
+#endif
+}
+// a * b and a + b, correctly rounded and never contracted into an FMA, even in a unit compiled with -fmad=true
+HK_HD float mul_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+HK_HD float add_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+// x / y, sqrt(x) and 1 / x correctly rounded even where the unit is compiled with -prec-div=false / -prec-sqrt=false
+HK_HD float div_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fdiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+HK_HD float sqrt_rn(float a) {
+#if defined(__CUDA_ARCH__)
+    return __fsqrt_rn(a);
+#else
+    return sqrtf(a);
+#endif
+}
+HK_HD float rcp_rn(float a) {
+#if defined(__CUDA_ARCH__)
+    return __frcp_rn(a);
+#else
+    return 1.0f / a;
 #endif
 }
 HK_HD float clampf(float x, float lo, float hi) { return fmin_(fmax_(x, lo), hi); }
 HK_HD float saturate(float x) { return clampf(x, 0.0f, 1.0f); }
-HK_HD float fract(float x) { return x - floorf(x); }
+HK_HD float fract(float x) { return canon_nan(x - floorf(x)); }
 HK_HD float signf(float x) { return (x > 0.0f) ? 1.0f : ((x < 0.0f) ? -1.0f : 0.0f); }
 HK_HD float mixf(float a, float b, float t) { return fmaf(b, t, a * (1.0f - t)); }
 HK_HD float sq(float x) { return x * x; }
-HK_HD float pow5(float x) { float x2 = x * x; return x2 * x2 * x; }
-HK_HD float pow16(float x) { x = x * x; x = x * x; x = x * x; return x * x; }
-HK_HD float pow025(float x) { return sqrtf(sqrtf(x)); }
+HK_HD float pow5(float x) { float x2 = x * x; return canon_nan(x2 * x2 * x); }
+HK_HD float pow16(float x) { x = x * x; x = x * x; x = x * x; return canon_nan(x * x); }
+HK_HD float pow025(float x) { return canon_nan(sqrtf(sqrtf(x))); }
 HK_HD bool is_nan(float v) { return !(v < 0.0f || 0.0f < v || v == 0.0f); }  // utils.wgsl:3-5
 
 // Exact integer -> float for 0 <= v < 2^23 by planting the integer in the mantissa of 2^23 (no I2F on the conversion pipe).
@@ -92,8 +149,6 @@ HK_HD float div_const(float x) {
     return fmaf(r, y, q);
 }
 
-HK_HD uint32_t f2u(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
-HK_HD float u2f(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
 
 // WGSL u32(f32): truncate toward zero, clamped to the u32 range (negative / NaN -> 0).
 HK_HD uint32_t f32_to_u32(float f) {
@@ -145,25 +200,27 @@ HK_HD float exp2_(float x) {
     int32_t e1 = e / 2, e2 = e - e1;
     return p * u2f((uint32_t)(e1 + 127) << 23) * u2f((uint32_t)(e2 + 127) << 23);
 }
-HK_HD float exp_(float x) { return exp2_(x * 1.4426950408889634f); }
+HK_HD float exp_(float x) { return exp2_(canon_nan(x * 1.4426950408889634f)); }
 
 // sin and cos together; intended range |x| <= ~1e3 (callers pass [0, 2*pi]).
 HK_HD void sincos_(float x, float* s_out, float* c_out) {
-    float kt = x * 0.6366197723675814f + 12582912.0f;   // x * 2/pi, rounded to nearest even (see exp2_)
-    float k = kt - 12582912.0f;
+    float kt = canon_nan(add_rn(mul_rn(x, 0.6366197723675814f), 12582912.0f));   // x * 2/pi, rounded to nearest even (see exp2_)
+    float k = add_rn(kt, -12582912.0f);
     float r = fmaf(-k, 1.5707962513e+0f, x);   // Cody-Waite, pi/2 split in three
     r = fmaf(-k, 7.5497894159e-8f, r);
     r = fmaf(-k, 5.3903029534e-15f, r);
-    float r2 = r * r;
+    float r2 = mul_rn(r, r);
     float sp = -1.9515295891e-4f;
     sp = fmaf(sp, r2, 8.3321608736e-3f);
     sp = fmaf(sp, r2, -1.6666654611e-1f);
-    float s = fmaf(sp * r2, r, r);
+    float s = fmaf(mul_rn(sp, r2), r, r);
     float cp = 2.443315711809948e-5f;
     cp = fmaf(cp, r2, -1.388731625493765e-3f);
     cp = fmaf(cp, r2, 4.166664568298827e-2f);
-    float c = fmaf(cp * r2, r2, fmaf(-0.5f, r2, 1.0f));
+    float c = fmaf(mul_rn(cp, r2), r2, fmaf(-0.5f, r2, 1.0f));
     int32_t q = ((int32_t)f2u(kt) - 0x4B400000) & 3;
+    s = canon_nan(s);
+    c = canon_nan(c);
     float sr = (q & 1) ? c : s;
     float cr = (q & 1) ? s : c;
     if (q & 2) sr = -sr;
@@ -223,8 +280,10 @@ HK_HD vec3 cross(vec3 a, vec3 b) {
 }
 HK_HD float length(vec3 a) { return sqrtf(dot(a, a)); }
 HK_HD float length(vec2 a) { return sqrtf(dot(a, a)); }
-HK_HD vec3 normalize(vec3 a) { float inv = 1.0f / sqrtf(dot(a, a)); return a * inv; }
-HK_HD vec2 normalize(vec2 a) { float inv = 1.0f / sqrtf(dot(a, a)); return a * inv; }
+HK_HD vec3 canon_nan(vec3 a) { return v3(canon_nan(a.x), canon_nan(a.y), canon_nan(a.z)); }
+// normalize(0) is 0 * inf: a NaN, 0x7FFFFFFF on the device
+HK_HD vec3 normalize(vec3 a) { float inv = 1.0f / sqrtf(dot(a, a)); return canon_nan(a * inv); }
+HK_HD vec2 normalize(vec2 a) { float inv = 1.0f / sqrtf(dot(a, a)); vec2 r = a * inv; return v2(canon_nan(r.x), canon_nan(r.y)); }
 HK_HD vec3 vmin(vec3 a, vec3 b) { return v3(fmin_(a.x, b.x), fmin_(a.y, b.y), fmin_(a.z, b.z)); }
 HK_HD vec3 vmax(vec3 a, vec3 b) { return v3(fmax_(a.x, b.x), fmax_(a.y, b.y), fmax_(a.z, b.z)); }
 HK_HD vec3 vmax(vec3 a, float s) { return v3(fmax_(a.x, s), fmax_(a.y, s), fmax_(a.z, s)); }
@@ -286,14 +345,16 @@ HK_HD float random_float(uint32_t value) { return (float)hash_u32(value) / 42949
 HK_HD uint16_t f32_to_f16_bits(float f) {
 #if defined(__CUDA_ARCH__)
     return __half_as_ushort(__float2half_rn(f));
-#elif defined(__F16C__)
+#else
+    if (f != f) return (uint16_t)0x7FFFu;           // cvt.rn.f16.f32 turns every NaN into the canonical 0x7FFF
+#if defined(__F16C__)
     return (uint16_t)_cvtss_sh(f, _MM_FROUND_TO_NEAREST_INT | _MM_FROUND_NO_EXC);
 #else
     uint32_t x = f2u(f);
     uint32_t sign = (x >> 16) & 0x8000u;
     uint32_t mant = x & 0x007FFFFFu;
     int32_t exp = (int32_t)((x >> 23) & 0xFF);
-    if (exp == 255) return (uint16_t)(sign | 0x7C00u | (mant ? (0x200u | (mant >> 13)) : 0u));
+    if (exp == 255) return (uint16_t)(sign | 0x7C00u);      // +-inf (NaN above)
     int32_t e = exp - 127 + 15;
     if (e >= 31) return (uint16_t)(sign | 0x7C00u);
     if (e <= 0) {
@@ -311,11 +372,14 @@ HK_HD uint16_t f32_to_f16_bits(float f) {
     if (rem > 0x1000u || (rem == 0x1000u && (half & 1u))) half++;
     return (uint16_t)(sign | half);
 #endif
+#endif
 }
 HK_HD float f16_bits_to_f32(uint16_t h) {
 #if defined(__CUDA_ARCH__)
     return __half2float(__ushort_as_half(h));
-#elif defined(__F16C__)
+#else
+    if ((h & 0x7C00u) == 0x7C00u && (h & 0x3FFu)) return u2f(0x7FFFFFFFu);   // cvt.f32.f16: every NaN becomes the canonical 0x7FFFFFFF
+#if defined(__F16C__)
     return _cvtsh_ss(h);
 #else
     uint32_t sign = ((uint32_t)h & 0x8000u) << 16;
@@ -326,8 +390,9 @@ HK_HD float f16_bits_to_f32(uint16_t h) {
         float m = (float)mant * 5.9604644775390625e-8f;  // 2^-24
         return (sign ? -m : m);
     }
-    if (exp == 31) return u2f(sign | 0x7F800000u | (mant << 13));
+    if (exp == 31) return u2f(sign | 0x7F800000u);          // +-inf (NaN above)
     return u2f(sign | ((exp + 112u) << 23) | (mant << 13));
+#endif
 #endif
 }
 HK_HD uint32_t pack2x16float(float a, float b) {
@@ -338,15 +403,15 @@ HK_HD vec2 unpack2x16float(uint32_t u) {
 }
 // WGSL spec: floor(0.5 + 65535 * min(1, max(0, e)))
 HK_HD uint32_t pack2x16unorm(float a, float b) {
-    uint32_t x = (uint32_t)floorf(0.5f + 65535.0f * fmin_(1.0f, fmax_(0.0f, a)));
-    uint32_t y = (uint32_t)floorf(0.5f + 65535.0f * fmin_(1.0f, fmax_(0.0f, b)));
+    uint32_t x = (uint32_t)floorf(add_rn(0.5f, mul_rn(65535.0f, fmin_(1.0f, fmax_(0.0f, a)))));
+    uint32_t y = (uint32_t)floorf(add_rn(0.5f, mul_rn(65535.0f, fmin_(1.0f, fmax_(0.0f, b)))));
     return x | (y << 16);
 }
 HK_HD vec2 unpack2x16unorm(uint32_t u) { return v2(div_const<65535>(u23_to_float(u & 0xFFFFu)), div_const<65535>(u23_to_float(u >> 16))); }
 HK_HD float unorm8(uint32_t b) { return div_const<255>(u23_to_float(b & 0xFFu)); }   // Rgba8Unorm texel component
 // WGSL spec: floor(0.5 + 127 * min(1, max(-1, e))), two's complement byte
 HK_HD uint32_t snorm8(float e) {
-    int32_t i = (int32_t)floorf(0.5f + 127.0f * fmin_(1.0f, fmax_(-1.0f, e)));
+    int32_t i = (int32_t)floorf(add_rn(0.5f, mul_rn(127.0f, fmin_(1.0f, fmax_(-1.0f, e)))));
     return (uint32_t)i & 0xFFu;
 }
 HK_HD uint32_t pack4x8snorm(vec4 v) {
@@ -369,13 +434,13 @@ HK_HD float D_GGX(float roughness, float NoH) {
     float oneMinusNoHSquared = 1.0f - NoH * NoH;
     float a = NoH * roughness;
     float k = roughness / (oneMinusNoHSquared + a * a);
-    return k * k * (1.0f / PI);
+    return canon_nan(k * k * (1.0f / PI));
 }
 HK_HD float V_SmithGGXCorrelated(float roughness, float NoV, float NoL) {
     float a2 = roughness * roughness;
     float lambdaV = NoL * sqrtf((NoV - a2 * NoV) * NoV + a2);
     float lambdaL = NoV * sqrtf((NoL - a2 * NoL) * NoL + a2);
-    return 0.5f / (lambdaV + lambdaL);
+    return canon_nan(0.5f / (lambdaV + lambdaL));
 }
 HK_HD vec3 F_Schlick_vec(vec3 f0, float f90, float VoH) {
     float p = pow5(1.0f - VoH);
@@ -404,13 +469,13 @@ HK_HD vec3 EnvBRDFApprox(vec3 f0, float perceptual_roughness, float NoV) {
     vec4 r = c0 * perceptual_roughness + c1;
     float a004 = fmin_(r.x * r.x, exp2_(-9.28f * NoV)) * r.x + r.y;
     vec2 AB = v2(-1.04f, 1.04f) * a004 + v2(r.z, r.w);
-    return f0 * AB.x + AB.y;
+    return canon_nan(f0 * AB.x + AB.y);
 }
 // bevy_core_pipeline::tonemapping
 HK_HD vec3 reinhard_luminance(vec3 color) {
     float l_old = luminance(color);
     float l_new = l_old / (1.0f + l_old);
-    return color * (l_new / l_old);
+    return canon_nan(color * (l_new / l_old));
 }
 
 // ------------------------------------------------------------------------------------ FSR 1.0 primitives

@@ -1145,6 +1145,24 @@ void pass_indirect(Ctx& c) {  // light.wgsl:1263-1498
 }
 
 // ----------------------------------------------------------------------------------- P4: spatial_reuse
+// Neighbour i of the pixel at `coords` (light.wgsl:1566-1575): its offset, its radius and its pixel
+inline ivec2 spatial_neighbour(ivec2 coords, uint32_t i, uint32_t count, float range, float rotation, float random_frame,
+                               float& rad, vec2& offset) {
+    float ang = TAU * fract((float)i * GOLDEN_RATIO + rotation + random_frame);
+    rad = sqrtf((float)i / (float)count) * range;
+    float sn, cs; sincos_(ang, &sn, &cs);
+    offset = rad * v2(cs, sn);
+    ivec2 sample_coords;
+    sample_coords.x = f32_to_i32(offset.x + (float)coords.x);
+    sample_coords.y = f32_to_i32(offset.y + (float)coords.y);
+    return sample_coords;
+}
+// uv of the depth-march tap at distance tap_dist towards that neighbour (light.wgsl:1617-1619)
+inline vec2 spatial_tap_uv(vec2 uv, vec2 offset, float tap_dist, ivec2 render_size) {
+    vec2 tap_offset = tap_dist * normalize(offset);
+    return uv + tap_offset / v2((float)render_size.x, (float)render_size.y);
+}
+
 template <bool EMISSIVE_LIT, bool RENDER_EMISSIVE>
 void pass_spatial_reuse(Ctx& c, int signal) {  // light.wgsl:1500-1684
     Deferred g(c);
@@ -1191,13 +1209,10 @@ void pass_spatial_reuse(Ctx& c, int signal) {  // light.wgsl:1500-1684
         r.s.visible_normal = s.visible_normal;
 
         for (uint32_t i = 1u; i <= SPATIAL_REUSE_COUNT; i += 1u) {
-            float ang = TAU * fract((float)i * GOLDEN_RATIO + sum4(s.random) + random_float(frame.number));
-            float rad = sqrtf((float)i / (float)SPATIAL_REUSE_COUNT) * SPATIAL_REUSE_RANGE;
-            float sn, cs; sincos_(ang, &sn, &cs);
-            vec2 offset = rad * v2(cs, sn);
-            ivec2 sample_coords;
-            sample_coords.x = f32_to_i32(offset.x + (float)coords.x);
-            sample_coords.y = f32_to_i32(offset.y + (float)coords.y);
+            float rad;
+            vec2 offset;
+            ivec2 sample_coords = spatial_neighbour(coords, i, SPATIAL_REUSE_COUNT, SPATIAL_REUSE_RANGE, sum4(s.random),
+                                                    random_float(frame.number), rad, offset);
             vec2 sample_uv = coords_to_uv(sample_coords, render_size);
             ivec2 sample_deferred_coords = g.jittered_coords(sample_uv);
             if (sample_uv.x < 0.0f || sample_uv.y < 0.0f || sample_uv.x > 1.0f || sample_uv.y > 1.0f) continue;
@@ -1216,10 +1231,7 @@ void pass_spatial_reuse(Ctx& c, int signal) {  // light.wgsl:1500-1684
             uint32_t tap_count = f32_to_u32(rad / tap_interval);
             bool occluded = false;
             for (uint32_t j = 1u; j <= tap_count; j += 1u) {
-                float tap_dist = (float)j * tap_interval;
-                vec2 tap_offset = tap_dist * normalize(offset);
-                vec2 tap_uv = uv + tap_offset / v2((float)render_size.x, (float)render_size.y);
-                ivec2 tap_deferred_coords = g.jittered_coords(tap_uv);
+                ivec2 tap_deferred_coords = g.jittered_coords(spatial_tap_uv(uv, offset, (float)j * tap_interval, render_size));
                 float tap_depth = g.position(tap_deferred_coords).w;
                 float ref_depth = mixf(depth, sample_depth, (float)j / (float)(tap_count + 1u));
                 if (tap_depth > ref_depth + 0.00001f) { occluded = true; break; }
@@ -2117,5 +2129,144 @@ void hko_math_normal_basis(const float* n, float* out9) {
     for (int i = 0; i < 3; ++i) { out9[3 * i] = m.c[i].x; out9[3 * i + 1] = m.c[i].y; out9[3 * i + 2] = m.c[i].z; }
 }
 void hko_pack_reservoir_roundtrip(const hk_packed_reservoir* in, hk_packed_reservoir* out) { *out = pack_reservoir(unpack_reservoir(*in)); }
+
+// Batch forms of the primitives for tests/test_gpu_device_math.py, which compares them with tests/cuda/math_probe.cu (the same
+// header compiled for the device): fn numbers as there.  hko_math_batch reads n inputs (2n for the two-operand functions);
+// hko_math_batch_range evaluates the bit patterns first .. first + n - 1.  fn 40 and above take and give several words per element
+// (normalize, the lighting functions, the reservoir record and its unpacked state).
+static uint32_t math_probe1(int fn, uint32_t u) {
+    const float x = u2f(u);
+    switch (fn) {
+        case 0: return f32_to_u32(x);
+        case 1: return (uint32_t)f32_to_i32(x);
+        case 2: return f32_to_f16_bits(x);
+        case 3: return snorm8(x);
+        case 4: return pack2x16unorm(x, 0.0f) & 0xFFFFu;
+        case 5: return f2u(fract(x));
+        case 6: return f2u(pow5(x));
+        case 7: return f2u(pow16(x));
+        case 8: return hash_u32(u);
+        case 9: { float s, c; sincos_(x, &s, &c); return f2u(s); }
+        case 10: { float s, c; sincos_(x, &s, &c); return f2u(c); }
+        case 11: return f2u(pow025(x));
+        case 12: return f2u(random_float(u));
+        case 13: return f2u(exp2_(x));
+        case 14: return f2u(exp_(x));
+        case 15: return f2u(saturate(x));
+        case 16: return f2u(f16_bits_to_f32((uint16_t)u));
+        case 17: return f2u(unsnorm8(u));
+        case 18: return f2u(unorm8(u));
+        case 19: return f2u(unpack2x16unorm(u).x);
+        default: return 0xDEADBEEFu;
+    }
+}
+static uint32_t math_probe2(int fn, uint32_t ua, uint32_t ub) {
+    const float a = u2f(ua), b = u2f(ub);
+    switch (fn) {
+        case 32: return f2u(fmin_(a, b));
+        case 33: return f2u(fmax_(a, b));
+        case 34: return f2u(clampf(a, b, 1.0f));
+        case 35: return f2u(clampf(a, -1.0f, b));
+        default: return 0xDEADBEEFu;
+    }
+}
+// fn 40..: several words in and out, as tests/cuda/math_probe.cu probe_words()
+static void math_probe_words(int fn, int& in, int& out) {
+    in = fn >= 32 ? 2 : 1; out = 1;
+    switch (fn) {
+        case 40: case 45: in = 3; out = 3; break;
+        case 41: in = 2; out = 2; break;
+        case 42: in = 2; break;
+        case 43: in = 3; break;
+        case 44: in = 5; out = 3; break;
+        case 50: in = 16; out = 16; break;
+        case 51: in = 16; out = 32; break;
+        case 52: in = 32; out = 16; break;
+        default: break;
+    }
+}
+static void math_probe_n(int fn, const uint32_t* a, uint32_t* o) {
+    auto f = [&](int k) { return u2f(a[k]); };
+    auto put3 = [&](vec3 r) { o[0] = f2u(r.x); o[1] = f2u(r.y); o[2] = f2u(r.z); };
+    hk_packed_reservoir p;
+    switch (fn) {
+        case 40: put3(normalize(v3(f(0), f(1), f(2)))); break;
+        case 41: { vec2 r = normalize(v2(f(0), f(1))); o[0] = f2u(r.x); o[1] = f2u(r.y); break; }
+        case 42: o[0] = f2u(D_GGX(f(0), f(1))); break;
+        case 43: o[0] = f2u(V_SmithGGXCorrelated(f(0), f(1), f(2))); break;
+        case 44: put3(EnvBRDFApprox(v3(f(0), f(1), f(2)), f(3), f(4))); break;
+        case 45: put3(reinhard_luminance(v3(f(0), f(1), f(2)))); break;
+        case 50: memcpy(&p, a, 64); p = pack_reservoir(unpack_reservoir(p)); memcpy(o, &p, 64); break;
+        case 51: {      // the unpacked state as 32 words (math_probe.cu P_UNPACK_RESERVOIR)
+            memcpy(&p, a, 64);
+            const Reservoir r = unpack_reservoir(p);
+            const float v[32] = {r.s.radiance.x, r.s.radiance.y, r.s.radiance.z, r.s.radiance.w, r.s.random.x, r.s.random.y, r.s.random.z,
+                                 r.s.random.w, r.s.visible_position.x, r.s.visible_position.y, r.s.visible_position.z, r.s.visible_position.w,
+                                 r.s.visible_normal.x, r.s.visible_normal.y, r.s.visible_normal.z, 0.0f, r.s.sample_position.x,
+                                 r.s.sample_position.y, r.s.sample_position.z, r.s.sample_position.w, r.s.sample_normal.x, r.s.sample_normal.y,
+                                 r.s.sample_normal.z, r.count, r.lifetime, r.w, r.w_sum, r.w2_sum, 0.0f, 0.0f, 0.0f, 0.0f};
+            for (int k = 0; k < 32; ++k) o[k] = f2u(v[k]);
+            o[15] = r.s.visible_instance;
+            break;
+        }
+        case 52: {
+            Reservoir r;
+            r.s.radiance = v4(f(0), f(1), f(2), f(3)); r.s.random = v4(f(4), f(5), f(6), f(7));
+            r.s.visible_position = v4(f(8), f(9), f(10), f(11)); r.s.visible_normal = v3(f(12), f(13), f(14));
+            r.s.visible_instance = a[15];
+            r.s.sample_position = v4(f(16), f(17), f(18), f(19)); r.s.sample_normal = v3(f(20), f(21), f(22));
+            r.count = f(23); r.lifetime = f(24); r.w = f(25); r.w_sum = f(26); r.w2_sum = f(27);
+            p = pack_reservoir(r);
+            memcpy(o, &p, 64);
+            break;
+        }
+        default: o[0] = 0xDEADBEEFu; break;
+    }
+}
+void hko_math_batch(int fn, const uint32_t* in, uint32_t* out, size_t n) {
+    int win, wout;
+    math_probe_words(fn, win, wout);
+#pragma omp parallel for schedule(static)
+    for (int64_t i = 0; i < (int64_t)n; ++i) {
+        if (fn >= 40) math_probe_n(fn, in + i * win, out + i * wout);
+        else out[i] = fn >= 32 ? math_probe2(fn, in[2 * i], in[2 * i + 1]) : math_probe1(fn, in[i]);
+    }
+}
+void hko_math_batch_range(int fn, uint32_t first, uint32_t* out, size_t n) {
+#pragma omp parallel for schedule(static)
+    for (int64_t i = 0; i < (int64_t)n; ++i) out[i] = math_probe1(fn, first + (uint32_t)i);
+}
+// Per pixel of a w x h frame at upscale ratio 1: an FNV-1a digest over the pixel of every spatial neighbour and the pixels of its
+// depth-march taps, as pass_spatial_reuse computes them (spatial_neighbour, spatial_tap_uv), for the rotation math_probe.cu draws
+void hko_spatial_digest(uint32_t count, float range, int w, int h, uint32_t frame, uint32_t* out) {
+    ivec2 size; size.x = w; size.y = h;
+    const float random_frame = random_float(frame);
+    const float tap_count_f = 4.0f + 1.0f;          // SPATIAL_REUSE_TAPS + 1
+#pragma omp parallel for schedule(static)
+    for (int64_t p = 0; p < (int64_t)w * h; ++p) {
+        ivec2 coords; coords.x = (int)(p % w); coords.y = (int)(p / w);
+        vec4 r;
+        float* c = &r.x;
+        for (uint32_t k = 0; k < 4u; ++k) c[k] = f16_bits_to_f32((uint16_t)(hash_u32((uint32_t)p * 4u + k + frame * 0x9E3779B9u) % 0x3C00u));
+        const float rotation = sum4(r);
+        const vec2 uv = coords_to_uv(coords, size);
+        uint32_t d = 2166136261u;
+        for (uint32_t i = 1u; i <= count; ++i) {
+            float rad;
+            vec2 offset;
+            ivec2 sc = spatial_neighbour(coords, i, count, range, rotation, random_frame, rad, offset);
+            d = (d ^ (uint32_t)sc.x) * 16777619u;
+            d = (d ^ (uint32_t)sc.y) * 16777619u;
+            float tap_interval = fmax_(1.0f, rad / tap_count_f);
+            uint32_t tap_count = f32_to_u32(rad / tap_interval);
+            for (uint32_t j = 1u; j <= tap_count; j += 1u) {
+                vec2 t = spatial_tap_uv(uv, offset, (float)j * tap_interval, size);   // jittered_coords at ratio 1: uv + 0
+                d = (d ^ (uint32_t)f32_to_i32(t.x * (float)w)) * 16777619u;
+                d = (d ^ (uint32_t)f32_to_i32(t.y * (float)h)) * 16777619u;
+            }
+        }
+        out[p] = d;
+    }
+}
 
 }  // extern "C"

@@ -68,6 +68,9 @@ def lib():
             "hko_math_unorm16": (C.c_float, [_U32]),
             "hko_math_normal_basis": (None, [_P, _P]),
             "hko_pack_reservoir_roundtrip": (None, [_P, _P]),
+            "hko_math_batch": (None, [_I, _P, _P, _SZ]),
+            "hko_math_batch_range": (None, [_I, _U32, _P, _SZ]),
+            "hko_spatial_digest": (None, [_U32, C.c_float, _I, _I, _U32, _P]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(_lib, name)

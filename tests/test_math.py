@@ -1,10 +1,62 @@
 """Known-answer tests of include/hk_math.h (through the oracle build of the same header): the arithmetic both the CUDA
 kernels and the oracle use.  Expected values come from numpy / the WGSL spec formulas, computed independently here."""
 import ctypes as C
+import os
+import shutil
+import subprocess
 
 import numpy as np
+import pytest
 
 from oracle import oracle
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+# the oracle's compiler and flags (oracle/Makefile), for the exhaustive host checks below
+HOST_CXX = ["/usr/bin/g++", "-O3", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fopenmp", "-fPIC", "-shared", "-std=c++17",
+            "-fvisibility=hidden", "-fvisibility-inlines-hidden", "-I", os.path.join(ROOT, "include")]
+
+# Every float in a range through the host build of hk_math.h, checked against float64 libm in C (numpy would take minutes)
+ACCURACY_SRC = r"""
+#define _GNU_SOURCE 1
+#include "hk_math.h"
+#include <math.h>
+static double ulp_of(double r) { int e; frexp(r, &e); return ldexp(1.0, e - 24 < -149 ? -149 : e - 24); }
+extern "C" __attribute__((visibility("default"))) double worst_exp2_ulp(uint32_t lo, uint32_t hi) {
+    double worst = 0.0;
+#pragma omp parallel for reduction(max : worst) schedule(static)
+    for (int64_t b = lo; b <= (int64_t)hi; ++b) {
+        const float x = hk::u2f((uint32_t)b);
+        const double r = exp2((double)x);
+        const double e = fabs((double)hk::exp2_(x) - r) / ulp_of(r);
+        worst = e > worst ? e : worst;
+    }
+    return worst;
+}
+extern "C" __attribute__((visibility("default"))) double worst_sincos_abs(uint32_t lo, uint32_t hi) {
+    double worst = 0.0;
+#pragma omp parallel for reduction(max : worst) schedule(static)
+    for (int64_t b = lo; b <= (int64_t)hi; ++b) {
+        const float x = hk::u2f((uint32_t)b);
+        float s, c;
+        double rs, rc;
+        hk::sincos_(x, &s, &c);
+        sincos((double)x, &rs, &rc);
+        const double e = fmax(fabs((double)s - rs), fabs((double)c - rc));
+        worst = e > worst ? e : worst;
+    }
+    return worst;
+}
+"""
+
+
+def compile_host(tmp_path, name, src, extra=()):
+    if not os.path.exists(HOST_CXX[0]):
+        pytest.skip("no host C++ compiler")
+    cpp, so = tmp_path / (name + ".cpp"), tmp_path / (name + ".so")
+    cpp.write_text(src)
+    r = subprocess.run(HOST_CXX + list(extra) + ["-o", str(so), str(cpp)], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    return C.CDLL(str(so))
 
 
 def ulp_diff(a, b):
@@ -13,13 +65,17 @@ def ulp_diff(a, b):
     return abs(ia - ib)
 
 
+def test_exp2_is_within_two_ulp_for_every_float_in_its_range(tmp_path):
+    """The bound include/hk_math.h states for exp2_, over every float in [-126, 128) against float64"""
+    acc = compile_host(tmp_path, "accuracy", ACCURACY_SRC)
+    acc.worst_exp2_ulp.restype, acc.worst_exp2_ulp.argtypes = C.c_double, [C.c_uint32, C.c_uint32]
+    worst = max(acc.worst_exp2_ulp(0x00000000, 0x42FFFFFF),      # +0 .. the float below 128
+                acc.worst_exp2_ulp(0x80000000, 0xC2FC0000))      # -0 .. -126
+    assert worst <= 2.0, worst
+
+
 def test_exp2_and_exp_accuracy():
     lib = oracle.lib()
-    xs = np.concatenate([np.linspace(-30, 30, 4001), np.linspace(-126, -100, 101), [0.0, 1.0, -1.0, 127.5]]).astype(np.float32)
-    worst = 0
-    for x in xs:
-        worst = max(worst, ulp_diff(lib.hko_math_exp2(float(x)), np.exp2(np.float64(x))))
-    assert worst <= 2, worst
     for x in np.linspace(-20, 5, 2001).astype(np.float32):
         # WGSL accuracy requirement for exp(x) is 3 + 2|x| ULP; exp_(x) = exp2_(x * log2(e)) stays far inside it
         assert ulp_diff(lib.hko_math_exp(float(x)), np.exp(np.float64(x))) <= 3 + 2 * abs(float(x))
@@ -27,12 +83,14 @@ def test_exp2_and_exp_accuracy():
     assert lib.hko_math_exp2(0.0) == 1.0 and lib.hko_math_exp2(10.0) == 1024.0
 
 
-def test_sincos_accuracy_over_the_range_the_path_uses():
+def test_sincos_accuracy_over_the_range_the_path_uses(tmp_path):
+    """Every float in [0, 2 pi] (the spatial pass's angles), against float64"""
+    acc = compile_host(tmp_path, "accuracy", ACCURACY_SRC)
+    acc.worst_sincos_abs.restype, acc.worst_sincos_abs.argtypes = C.c_double, [C.c_uint32, C.c_uint32]
+    worst = acc.worst_sincos_abs(0x00000000, int(np.float32(2 * np.pi).view(np.uint32)))
+    assert worst < 3e-7, worst
     lib = oracle.lib()
     s, c = C.c_float(), C.c_float()
-    for x in np.linspace(0.0, 2 * np.pi, 5001).astype(np.float32):
-        lib.hko_math_sincos(float(x), C.byref(s), C.byref(c))
-        assert abs(s.value - np.sin(np.float64(x))) < 3e-7 and abs(c.value - np.cos(np.float64(x))) < 3e-7
     lib.hko_math_sincos(0.0, C.byref(s), C.byref(c))
     assert (s.value, c.value) == (0.0, 1.0)
 
@@ -186,3 +244,37 @@ def test_brdf_matches_float64_restatement_of_the_published_formulas():
     assert worst < 2e-5, worst
     assert lib.hko_math_perceptual_roughness_to_roughness(C.c_float(0.5)) == np.float32(0.25)
     assert lib.hko_math_perceptual_roughness_to_roughness(C.c_float(0.01)) == np.float32(np.float32(0.089) * np.float32(0.089))
+
+
+F16_SRC = r"""
+#include "hk_math.h"
+extern "C" __attribute__((visibility("default"))) void to_f16(uint32_t first, uint16_t* out, size_t n) {
+#pragma omp parallel for schedule(static)
+    for (int64_t i = 0; i < (int64_t)n; ++i) out[i] = hk::f32_to_f16_bits(hk::u2f(first + (uint32_t)i));
+}
+extern "C" __attribute__((visibility("default"))) void from_f16(uint32_t* out) {
+    for (uint32_t h = 0; h < 65536u; ++h) out[h] = hk::f2u(hk::f16_bits_to_f32((uint16_t)h));
+}
+"""
+
+
+def test_portable_f16_conversion_equals_the_f16c_one_for_every_input(tmp_path):
+    """include/hk_math.h has a portable f32 <-> f16 branch for hosts without F16C; it must be the same function as the F16C one
+    the oracle is built with: all 2^32 floats to f16 and all 2^16 halves back"""
+    f16c = compile_host(tmp_path, "f16c", F16_SRC)
+    portable = compile_host(tmp_path, "portable", F16_SRC, ["-mno-f16c"])
+    for lib in (f16c, portable):
+        lib.to_f16.restype, lib.to_f16.argtypes = None, [C.c_uint32, C.c_void_p, C.c_size_t]
+        lib.from_f16.restype, lib.from_f16.argtypes = None, [C.c_void_p]
+    a, b = np.empty(65536, np.uint32), np.empty(65536, np.uint32)
+    f16c.from_f16(a.ctypes.data)
+    portable.from_f16(b.ctypes.data)
+    bad = np.flatnonzero(a != b)
+    assert bad.size == 0, [(hex(h), hex(a[h]), hex(b[h])) for h in bad[:8]]
+    n = 1 << 28
+    a, b = np.empty(n, np.uint16), np.empty(n, np.uint16)
+    for first in range(0, 1 << 32, n):
+        f16c.to_f16(first, a.ctypes.data, n)
+        portable.to_f16(first, b.ctypes.data, n)
+        bad = np.flatnonzero(a != b)
+        assert bad.size == 0, [(hex(first + int(i)), hex(a[i]), hex(b[i])) for i in bad[:8]]

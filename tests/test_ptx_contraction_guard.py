@@ -1,0 +1,60 @@
+"""Contraction guard, CPU only: the arithmetic that ends in an integer must stay exact in the tolerance units.
+
+build.py compiles kernels_spatial.cu and kernels_post.cu with -fmad=true -prec-div=false -prec-sqrt=false (FAST_FLAGS).  Under
+those flags nvcc fuses a plain a * b + c into one FMA and ptxas may fuse a `mul.f32` / `add.f32` pair that carries no rounding
+modifier.  sincos_, snorm8, pack2x16unorm (include/hk_math.h), pack_reservoir (csrc/hk_device.cuh) and the spatial-reuse pixel
+helpers (csrc/hk_spatial_taps.cuh) feed f32 -> integer conversions, where one rounding step decides a neighbour, a stored normal
+byte or a lifetime, so they write every product and sum as mul_rn / add_rn (.rn in the PTX: never fused) and every quotient and
+square root as div_rn / sqrt_rn / rcp_rn.  This test cross-compiles each of them alone with the tolerance flags and reads the PTX:
+  * no f32 mul / add / sub without .rn, no approximate division, square root or reciprocal;
+  * exactly as many FMAs as the exact flags give (the explicit fmaf() calls): none was contracted.
+tests/test_gpu_device_math.py checks the same functions bit for bit on the H100; this keeps them from regressing between GPU runs."""
+import os
+import re
+import subprocess
+
+import pytest
+
+from bevy_hikari_b200 import build as product_build
+
+SNIPPETS = {
+    "sincos_": "float s, c; hk::sincos_(i[0], &s, &c); o[0] = s; o[1] = c;",
+    "snorm8": "u[0] = hk::snorm8(i[0]);",
+    "pack_reservoir": "hkd::Reservoir r = hkd::zero_reservoir(); r.lifetime = i[0]; r.s.visible_normal = hk::v3(i[1], i[2], i[3]); "
+                      "r.s.random = hk::v4(i[4], i[5], i[6], i[7]); hkd::PackedQuarters p = hkd::pack_reservoir(r); "
+                      "u[0] = p.q3.x; u[1] = p.q0.z; u[2] = p.q0.w;",
+    "pack2x16unorm": "u[0] = hk::pack2x16unorm(i[0], i[1]);",
+    "spatial_neighbour": "hk::vec2 off = hkd::spatial_offset(i[0], i[1], i[2], i[3]); int sx, sy; "
+                         "hkd::spatial_neighbour_pixel(off, n[0], n[1], sx, sy); u[0] = sx; u[1] = sy; o[0] = off.x; o[1] = off.y;",
+    "spatial_march_tap": "hk::vec2 uv = hkd::spatial_pixel_uv(n[0], n[1], i[4], i[5]); "
+                         "hk::vec2 unit = hkd::spatial_march_unit(hk::v2(i[0], i[1])); int tx, ty; "
+                         "hkd::spatial_tap_pixel(hkd::spatial_tap_uv(uv, unit, i[2], i[4], i[5], i[6], i[7]), n[2], n[3], tx, ty); "
+                         "u[0] = tx; u[1] = ty;",
+}
+SOURCE = """#include "hk_device.cuh"
+#include "hk_spatial_taps.cuh"
+extern "C" __global__ void probe(const float* i, const int* n, float* o, unsigned* u) { %s }
+"""
+
+
+def ptx(tmp_path, name, body, flavor):
+    src = tmp_path / f"{name}.cu"
+    out = tmp_path / f"{name}.{flavor}.ptx"
+    src.write_text(SOURCE % body)
+    flags = [f for f in product_build.probe_flags(flavor) if f != "-lineinfo"]
+    r = subprocess.run([product_build.NVCC] + flags + ["-ptx", str(src), "-o", str(out)], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    return out.read_text()
+
+
+@pytest.mark.parametrize("name", sorted(SNIPPETS))
+def test_integer_feeding_arithmetic_is_never_contracted_or_approximated(tmp_path, name):
+    if not os.path.exists(product_build.NVCC):
+        pytest.skip("no nvcc")
+    fast, exact = ptx(tmp_path, name, SNIPPETS[name], "fast"), ptx(tmp_path, name, SNIPPETS[name], "exact")
+    plain = re.findall(r"^\s*(?:mul|add|sub)\.f32\s.*$", fast, re.M)
+    assert not plain, f"{name}: f32 arithmetic without .rn in the tolerance build: {plain[:4]}"
+    approx = re.findall(r"^\s*(?:div\.(?:approx|full)|sqrt\.approx|rsqrt|rcp\.approx)\S*\s.*$", fast, re.M)
+    assert not approx, f"{name}: approximate division / square root in the tolerance build: {approx[:4]}"
+    fma = lambda text: len(re.findall(r"^\s*fma\.rn\.f32\s", text, re.M))
+    assert fma(fast) == fma(exact), f"{name}: {fma(fast)} FMAs with the tolerance flags, {fma(exact)} with the exact ones"

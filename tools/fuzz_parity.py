@@ -20,6 +20,20 @@ from tests.conftest import Animation, Bench, rotation_y_about  # noqa: E402
 from tests.test_gpu_parity import ALL_PLANES, DENOISED, mismatch  # noqa: E402
 
 
+def draw_tuning(seed):
+    """hk_set_tuning switches that leave every output bit-exact: pooled indirect pass, tiled or gathered spatial reuse, tiled or
+    gathered denoise.  From a stream of its own, so that a seed still draws the scene, size and settings it always drew."""
+    rng = np.random.default_rng(seed + 2 ** 20)
+    return {plugin.TUNE_POOLED_INDIRECT: int(rng.integers(0, 2)), plugin.TUNE_TILED_SPATIAL: int(rng.integers(0, 2)),
+            plugin.TUNE_TILED_DENOISE: int(rng.integers(0, 2))}
+
+
+def apply_tuning(devices, tuning):
+    for d in devices:
+        for k, v in tuning.items():
+            d.set_tuning(k, v)
+
+
 def one_case(seed):
     rng = np.random.default_rng(seed)
     scene = rng.choice(["cornell", "cornell", "city", "simple", "minimal"])
@@ -42,6 +56,8 @@ def one_case(seed):
     b = Bench(str(scene), w, h, **settings)
     dev, orc = b.device(), b.oracle()
     dev.set_keep_intermediates(True)
+    tuning = draw_tuning(seed)
+    apply_tuning([dev], tuning)
     step = tuple(rng.uniform(-0.08, 0.08, 3)) if rng.integers(0, 2) else (0.0, 0.0, 0.0)
     an = None
     if rng.integers(0, 2):
@@ -67,7 +83,7 @@ def one_case(seed):
         bad = {k: mismatch(dev.readback(k), orc.readback(k)) for k in planes}
         bad = {k: v for k, v in bad.items() if v}
         if bad:
-            return f"seed {seed}: {scene} {w}x{h} frame {f} {settings} upscalers={upscalers} step={step} animated={an is not None} -> {bad}"
+            return f"seed {seed}: {scene} {w}x{h} frame {f} {settings} upscalers={upscalers} step={step} animated={an is not None} tuning={tuning} -> {bad}"
     return None
 
 
@@ -85,6 +101,8 @@ def tile_case(seed):
     rects = [(x0, x1, y0, y1) for x0, x1 in zip(xs[:-1], xs[1:]) for y0, y1 in zip(ys[:-1], ys[1:])]
     full = b.device()
     tiles = [b.device(r[2], r[3], r[0], r[1]) for r in rects]
+    tuning = draw_tuning(seed)
+    apply_tuning([full] + tiles, tuning)
     halo = bool(os.environ.get("HK_FUZZ_HALO"))       # moving camera + motion margin + halo pulls after every frame
     step = tuple(rng.uniform(-0.05, 0.05, 3)) if halo else (0.0, 0.0, 0.0)
     upscalers = halo and bool(rng.integers(0, 2))     # ... and the temporal upscalers on the tiles
@@ -117,12 +135,12 @@ def tile_case(seed):
             whole = full.readback(k)
             for r, t in zip(rects, tiles):
                 if mismatch(t.readback(k), whole[r[2]:r[3], r[0]:r[1]]):
-                    return f"tile seed {seed}: {scene} {w}x{h} rects {rects} frame {f} plane {k} {settings}"
+                    return f"tile seed {seed}: {scene} {w}x{h} rects {rects} frame {f} plane {k} {settings} tuning={tuning}"
         for k, sc in scaled:
             whole = full.readback(k)
             for r, t in zip(rects, tiles):
                 if mismatch(t.readback(k), whole[sc * r[2]:sc * r[3], sc * r[0]:sc * r[1]]):
-                    return f"tile seed {seed}: {scene} {w}x{h} rects {rects} frame {f} upscaled plane {k} {settings}"
+                    return f"tile seed {seed}: {scene} {w}x{h} rects {rects} frame {f} upscaled plane {k} {settings} tuning={tuning}"
     return None
 
 
