@@ -8,7 +8,8 @@
                       denoise, tone mapping, upscalers' neighbours in kernels_post.cu / kernels_spatial.cu) are compiled with
                       FMA contraction and approximate division / square root / exp (FAST_FLAGS); everything that walks the BVH
                       or writes an id keeps exact arithmetic.  Contract: ids and temporal reservoirs bit-exact, radiance within
-                      1 f16 ulp per pass from identical inputs, < 1e-4 outlier pixels (tests/test_gpu_tolerance.py).
+                      1 f16 ulp per pass from identical inputs, < 1e-4 outlier pixels (tests/test_gpu_tolerance.py, and
+                      tests/test_gpu_tolerance_upscaled.py at upscale ratios above 1).
   libhikari_b200_exact.so   the same sources with exact arithmetic everywhere: bit-identical to the CPU oracle on every plane
                       (the 0-ulp parity suite runs on it).  Shares every object file with the product except the two above.
 

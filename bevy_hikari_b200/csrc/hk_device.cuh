@@ -860,26 +860,35 @@ __device__ __forceinline__ vec4 noise_random(const KParams& P, int x, int y) {
 }
 
 // ---- render space <-> deferred (G-buffer) space, light.wgsl:1007-1017 and denoise.wgsl:37-41
+// These end in an integer texel, and at upscale ratio 1.5 (sizes divisible by 3) half the columns and rows sit exactly on a texel
+// edge, so one rounding step picks another texel.  Every product, sum and quotient is therefore written as a correctly rounded operation (mul_rn /
+// add_rn / div_rn / rcp_rn): the operations the exact build emits anyway, never contracted or approximated in the tolerance build
+// (kernels_spatial.cu, kernels_post.cu), whose texels are then the oracle's too (tests/test_gpu_device_math.py).
 __device__ __forceinline__ vec2 render_uv(const KParams& P, int x, int y) {   // coords_to_uv(coords, render_size)
-    return (v2((float)x, (float)y) + 0.5f) / v2((float)P.band.RW, (float)P.band.RH);
+    return v2(div_rn(add_rn((float)x, 0.5f), (float)P.band.RW), div_rn(add_rn((float)y, 0.5f), (float)P.band.RH));
 }
 __device__ __forceinline__ vec2 jittered_deferred_uv(const KParams& P, vec2 uv, float amount) {
     if (P.ratio1) return uv;   // + (+-amount) * texel * 0
-    vec2 texel_size = v2(1.0f, 1.0f) / v2((float)P.band.W, (float)P.band.H);
-    return uv + (P.jitter_sign * amount) * texel_size * P.ratio_m1;
+    const float s = mul_rn(P.jitter_sign, amount);     // uv + (+-amount) * texel_size * (ratio - 1), texel_size = 1 / size
+    return v2(add_rn(uv.x, mul_rn(mul_rn(s, rcp_rn((float)P.band.W)), P.ratio_m1)),
+              add_rn(uv.y, mul_rn(mul_rn(s, rcp_rn((float)P.band.H)), P.ratio_m1)));
 }
-// jittered_deferred_coords (light passes: +-0.25 texel, truncation); (x, y) is the render pixel whose uv is `uv`
+// jittered_deferred_coords (light passes: +-0.25 texel, truncation) of any uv: a pixel's, a neighbour's or a depth-march tap's
+__device__ __forceinline__ void jittered_deferred_coords(const KParams& P, vec2 uv, int& dx, int& dy) {
+    const vec2 d = jittered_deferred_uv(P, uv, 0.25f);
+    dx = f32_to_i32(mul_rn(d.x, (float)P.band.W)); dy = f32_to_i32(mul_rn(d.y, (float)P.band.H));
+}
+// the same for the render pixel (x, y) whose uv is `uv`
 __device__ __forceinline__ void light_deferred_coords(const KParams& P, vec2 uv, int x, int y, int& dx, int& dy) {
     if (P.ratio1) { dx = x; dy = y; return; }   // trunc(((x + 0.5) / W) * W) == x
-    vec2 d = jittered_deferred_uv(P, uv, 0.25f);
-    dx = f32_to_i32(d.x * (float)P.band.W); dy = f32_to_i32(d.y * (float)P.band.H);
+    jittered_deferred_coords(P, uv, dx, dy);
 }
 // textureSampleLevel(<deferred texture>, nearest_sampler, jittered_deferred_uv(uv)) of the denoise passes: +-0.5 texel, floor, clamp
 __device__ __forceinline__ void denoise_deferred_coords(const KParams& P, vec2 uv, int x, int y, int& dx, int& dy) {
     if (P.ratio1) { dx = x; dy = y; return; }
     vec2 d = jittered_deferred_uv(P, uv, 0.5f);
-    dx = min(max((int)floorf(d.x * (float)P.band.W), 0), P.band.W - 1);
-    dy = min(max((int)floorf(d.y * (float)P.band.H), 0), P.band.H - 1);
+    dx = min(max((int)floorf(mul_rn(d.x, (float)P.band.W)), 0), P.band.W - 1);
+    dy = min(max((int)floorf(mul_rn(d.y, (float)P.band.H)), 0), P.band.H - 1);
 }
 __device__ __forceinline__ bool render_allocated(const KParams& P, int x, int y) {
     return P.ratio1 ? band_allocated(P.band, x, y) : (x >= 0 && x < P.band.RW && y >= 0 && y < P.band.RH);
@@ -900,12 +909,13 @@ __device__ __forceinline__ PassBuffers bind(const KParams& P, int signal) {
     b.spatial_reservoir = P.planes.reservoir[previous + spatial];
     return b;
 }
-// reprojected pixel of `previous_uv` (light.wgsl:181-190): returns false when outside [0,1) or outside the band
+// reprojected pixel of `previous_uv` (light.wgsl:181-190): returns false when outside [0,1) or outside the band.  Correctly rounded
+// like the deferred coordinates above (uv - 0.5 == uv + -0.5 exactly)
 __device__ __forceinline__ bool previous_pixel(const KParams& P, vec2 previous_uv, bool inclusive, size_t& pidx) {
-    float ax = fabsf(previous_uv.x - 0.5f), ay = fabsf(previous_uv.y - 0.5f);
+    float ax = fabsf(add_rn(previous_uv.x, -0.5f)), ay = fabsf(add_rn(previous_uv.y, -0.5f));
     bool inside = inclusive ? (ax <= 0.5f && ay <= 0.5f) : (ax < 0.5f && ay < 0.5f);
     if (!inside) return false;
-    int px = f32_to_i32(previous_uv.x * (float)P.band.RW), py = f32_to_i32(previous_uv.y * (float)P.band.RH);
+    int px = f32_to_i32(mul_rn(previous_uv.x, (float)P.band.RW)), py = f32_to_i32(mul_rn(previous_uv.y, (float)P.band.RH));
     if (!render_allocated(P, px, py)) return false;
     pidx = render_index(P.band, px, py);
     return true;

@@ -2,11 +2,11 @@
 // screen-space depth-march taps.  Both end in an integer pixel, so a rounding difference here is a different neighbour, not a
 // small radiance error.  Every product, sum, quotient and square root is written as a correctly rounded operation (hk::mul_rn,
 // hk::add_rn, hk::div_rn, hk::rcp_rn, hk::sqrt_rn: __fmul_rn, __fadd_rn, __fdiv_rn, __frcp_rn, __fsqrt_rn on the device), which
-// nvcc never contracts or approximates.  So at upscale ratio 1 (kc_spatial, and k_spatial when tiles are off) the spatial pass
-// picks the oracle's pixels (oracle/hk_oracle.cpp spatial_neighbour / spatial_tap_uv) in the tolerance build (-fmad=true,
-// -prec-div=false, -prec-sqrt=false) as well as in the exact one.  Above ratio 1, k_spatial maps the neighbour and each tap to a
-// G-buffer texel with the jittered uv of hk_device.cuh, which the tolerance build may still round differently.
-// tests/cuda/math_probe.cu runs these functions for every pixel of a frame.
+// nvcc never contracts or approximates.  So the spatial pass picks the oracle's pixels (oracle/hk_oracle.cpp spatial_neighbour /
+// spatial_tap_uv) in the tolerance build (-fmad=true, -prec-div=false, -prec-sqrt=false) as well as in the exact one.  Above upscale
+// ratio 1, k_spatial maps the neighbour and each tap to a G-buffer texel with jittered_deferred_coords of hk_device.cuh, written
+// the same way, so those texels are the oracle's too.  tests/cuda/math_probe.cu runs these functions for every pixel of a frame, at
+// ratio 1 and above it.
 #pragma once
 #include "hk_math.h"
 

@@ -100,7 +100,7 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_SPATIAL) k_spatial(const 
     const vec2 size_f = v2((float)P.band.RW, (float)P.band.RH);
     const SpatialTable& T = P.spatial_tables[EMISSIVE_LIT ? 1 : 0];
     const float rotation = sum4(s.random);
-    const vec2 march_uv = spatial_pixel_uv(x, y, size_f.x, size_f.y);     // = uv, rounded the oracle's way in the tolerance build too
+    const vec2 march_uv = spatial_pixel_uv(x, y, size_f.x, size_f.y);     // = uv (render_uv), the same correctly rounded quotients
     for (uint32_t i = 1u; i <= SPATIAL_REUSE_COUNT; i += 1u) {
         const vec2 offset = spatial_offset(T.phase[i], T.radius[i], rotation, P.random_frame);
         int sx, sy;
@@ -138,9 +138,8 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_SPATIAL) k_spatial(const 
         bool occluded = false;
         const vec2 unit = spatial_march_unit(offset);
         for (uint32_t j = 1u; j <= tap_count; j += 1u) {
-            vec2 tap_uv = spatial_tap_uv(march_uv, unit, T.tap_dist[i][j - 1u], size_f.x, size_f.y, P.inv_rw, P.inv_rh);
-            vec2 tap_deferred_uv = jittered_deferred_uv(P, tap_uv, 0.25f);
-            int tx = f32_to_i32(tap_deferred_uv.x * (float)P.band.W), ty = f32_to_i32(tap_deferred_uv.y * (float)P.band.H);
+            int tx, ty;
+            jittered_deferred_coords(P, spatial_tap_uv(march_uv, unit, T.tap_dist[i][j - 1u], size_f.x, size_f.y, P.inv_rw, P.inv_rh), tx, ty);
             float tap_depth = 0.0f;  // out-of-bounds textureLoad -> 0
             if (tx >= 0 && tx < P.band.W && ty >= 0 && ty < P.band.H) tap_depth = P.planes.pos_depth[band_index(P.band, tx, ty)].w;
             float ref_depth = mixf(depth, sample_depth, T.tap_ratio[i][j - 1u]);
@@ -282,8 +281,9 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
     const float4 vu = P.planes.velocity_uv[idx];
     const Surface surface = retreive_surface(sc, f32_to_u32(imf.y), v2(vu.z, vu.w));
     const bool use_spatial_variance = r.count <= 4.0f;
-    const vec2 uv = pixel_uv(P, x, y);
-    const vec2 previous_uv = uv - v2(vu.x, vu.y);       // jittered_deferred_uv is the identity at ratio 1
+    const vec2 size_f = v2((float)P.band.RW, (float)P.band.RH);
+    const vec2 march_uv = spatial_pixel_uv(x, y, size_f.x, size_f.y);     // = pixel_uv, the pixel's uv for the reprojection and the march
+    const vec2 previous_uv = march_uv - v2(vu.x, vu.y);     // jittered_deferred_uv is the identity at ratio 1
 
     Reservoir q = r;
     const Sample s = q.s;
@@ -304,9 +304,7 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
     r.s.visible_position = s.visible_position;
     r.s.visible_normal = s.visible_normal;
 
-    const vec2 size_f = v2((float)P.band.RW, (float)P.band.RH);
     const float rotation = sum4(s.random);
-    const vec2 march_uv = spatial_pixel_uv(x, y, size_f.x, size_f.y);     // = uv, rounded the oracle's way in the tolerance build too
     mbar_wait(s_bar, 0u);                               // the tiles have landed
 
     // Stage A, shared memory only: every test that rejects a neighbour without its gathered quarters — bounds, depth ratio, count

@@ -2268,5 +2268,77 @@ void hko_spatial_digest(uint32_t count, float range, int w, int h, uint32_t fram
         out[p] = d;
     }
 }
+// Per render pixel of a w x h frame at upscale ratio `ratio` in (1, 2]: four FNV-1a digests (math_probe.cu k_deferred_digest) of
+//   [0] the light passes' G-buffer texel, Deferred::jittered_coords of coords_to_uv,
+//   [1] the denoise passes' texel, Deferred::nearest of jittered_uv(uv, 0.5),
+//   [2] load_previous's pixel of jittered_uv(uv, 0.25) - velocity, with the all(< 0.5) and the all(<= 0.5) test (scatter), for
+//       velocity 0 and for the velocity math_probe.cu draws: the index, or ~0 outside.  A uv of exactly 1 passes the inclusive test
+//       with a pixel one past the row, which the device rejects: it counts as outside here too,
+//   [3] for both tables, pass_spatial_reuse's neighbour pixels (spatial_neighbour), the texel of each one inside the frame and of each
+//       of its depth-march taps (spatial_tap_uv).
+void hko_deferred_digest(int w, int h, float ratio, uint32_t frame, uint32_t* out) {
+    hko_context c;                  // what Deferred reads: the G-buffer size and the frame's upscale ratio and number
+    c.W = w; c.H = h;
+    memset(&c.in, 0, sizeof(c.in));
+    c.in.frame.upscale_ratio = ratio;
+    c.in.frame.number = frame;
+    const float scale = 1.0f / ratio;       // begin()
+    c.RW = (int)ceilf(scale * (float)c.W);
+    c.RH = (int)ceilf(scale * (float)c.H);
+    const Deferred g(c);
+    ivec2 size; size.x = c.RW; size.y = c.RH;
+    const float random_frame = random_float(frame);
+    const float tap_count_f = 4.0f + 1.0f;          // SPATIAL_REUSE_TAPS + 1
+    auto fnv = [](uint32_t d, uint32_t v) { return (d ^ v) * 16777619u; };
+#pragma omp parallel for schedule(static)
+    for (int64_t p = 0; p < (int64_t)size.x * size.y; ++p) {
+        ivec2 coords; coords.x = (int)(p % size.x); coords.y = (int)(p / size.x);
+        const vec2 uv = coords_to_uv(coords, size);
+        uint32_t d[4] = {2166136261u, 2166136261u, 2166136261u, 2166136261u};
+        ivec2 t = g.jittered_coords(uv);
+        d[0] = fnv(fnv(d[0], (uint32_t)t.x), (uint32_t)t.y);
+        t = g.nearest(g.jittered_uv(uv, 0.5f));
+        d[1] = fnv(fnv(d[1], (uint32_t)t.x), (uint32_t)t.y);
+        const uint32_t hv = hash_u32((uint32_t)p * 2u + frame * 0x85EBCA6Bu), gv = hash_u32(hv);       // math_probe.cu probe_velocity
+        const vec2 velocities[2] = {v2(0.0f, 0.0f), v2((float)((int)(hv & 0x3FFFu) - 0x2000) * 0x1p-16f,
+                                                       (float)((int)(gv & 0x3FFFu) - 0x2000) * 0x1p-16f)};
+        for (const vec2& velocity : velocities) {
+            const vec2 previous_uv = g.jittered_uv(uv, 0.25f) - v2(velocity.x, velocity.y);
+            for (int inclusive = 0; inclusive < 2; ++inclusive) {
+                uint32_t index = 0xFFFFFFFFu;
+                if (inclusive ? uv_inside_eq(previous_uv) : uv_inside(previous_uv)) {
+                    const bool in_frame = f32_to_i32(previous_uv.x * (float)size.x) < size.x && f32_to_i32(previous_uv.y * (float)size.y) < size.y;
+                    if (in_frame) index = (uint32_t)uv_to_index(previous_uv, size);
+                }
+                d[2] = fnv(d[2], index);
+            }
+        }
+        vec4 r;
+        float* rc = &r.x;
+        for (uint32_t k = 0; k < 4u; ++k) rc[k] = f16_bits_to_f32((uint16_t)(hash_u32((uint32_t)p * 4u + k + frame * 0x9E3779B9u) % 0x3C00u));
+        const float rotation = sum4(r);
+        const uint32_t counts[2] = {16u, 8u};
+        const float ranges[2] = {20.0f, 10.0f};
+        for (int table = 0; table < 2; ++table) {
+            for (uint32_t i = 1u; i <= counts[table]; ++i) {
+                float rad;
+                vec2 offset;
+                const ivec2 sc = spatial_neighbour(coords, i, counts[table], ranges[table], rotation, random_frame, rad, offset);
+                d[3] = fnv(fnv(d[3], (uint32_t)sc.x), (uint32_t)sc.y);
+                const vec2 sample_uv = coords_to_uv(sc, size);
+                if (sample_uv.x < 0.0f || sample_uv.y < 0.0f || sample_uv.x > 1.0f || sample_uv.y > 1.0f) continue;
+                t = g.jittered_coords(sample_uv);
+                d[3] = fnv(fnv(d[3], (uint32_t)t.x), (uint32_t)t.y);
+                const float tap_interval = fmax_(1.0f, rad / tap_count_f);
+                const uint32_t tap_count = f32_to_u32(rad / tap_interval);
+                for (uint32_t j = 1u; j <= tap_count; j += 1u) {
+                    t = g.jittered_coords(spatial_tap_uv(uv, offset, (float)j * tap_interval, size));
+                    d[3] = fnv(fnv(d[3], (uint32_t)t.x), (uint32_t)t.y);
+                }
+            }
+        }
+        for (int k = 0; k < 4; ++k) out[4 * p + k] = d[k];
+    }
+}
 
 }  // extern "C"

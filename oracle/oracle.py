@@ -71,6 +71,7 @@ def lib():
             "hko_math_batch": (None, [_I, _P, _P, _SZ]),
             "hko_math_batch_range": (None, [_I, _U32, _P, _SZ]),
             "hko_spatial_digest": (None, [_U32, C.c_float, _I, _I, _U32, _P]),
+            "hko_deferred_digest": (None, [_I, _I, C.c_float, _U32, _P]),
         }
         for name, (res, args) in sig.items():
             fn = getattr(_lib, name)

@@ -2,10 +2,11 @@
 //
 // build.py's build_math_probe() compiles this file twice, with the flags of the units that trace rays (libhk_math_probe_exact.so)
 // and with those of the tolerance units (libhk_math_probe_fast.so).  The test runs the same inputs through the oracle's build of
-// the header (hko_math_batch / hko_math_batch_range / hko_spatial_digest in oracle/hk_oracle.cpp) and compares the bits.  The
-// function numbers are shared with that file and with the test.
+// the header (hko_math_batch / hko_math_batch_range / hko_spatial_digest / hko_deferred_digest in oracle/hk_oracle.cpp) and compares
+// the bits.  The function numbers are shared with that file and with the test.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "hk_device.cuh"
 #include "hk_math.h"
@@ -170,6 +171,83 @@ __global__ void k_spatial_digest(const __grid_constant__ ProbeTable T, uint32_t 
     out[p] = d;
 }
 
+__host__ __device__ __forceinline__ uint32_t fnv(uint32_t d, uint32_t v) { return (d ^ v) * 16777619u; }
+
+// The velocity a pixel brings to the reprojection: multiples of 2^-16 in [-1/8, 1/8) drawn from a hash of pixel and frame
+__host__ __device__ __forceinline__ vec2 probe_velocity(uint32_t pixel, uint32_t frame) {
+    const uint32_t h = hash_u32(pixel * 2u + frame * 0x85EBCA6Bu), g = hash_u32(h);
+    return v2(mul_rn((float)((int)(h & 0x3FFFu) - 0x2000), 0x1p-16f), mul_rn((float)((int)(g & 0x3FFFu) - 0x2000), 0x1p-16f));
+}
+
+// Per render pixel at an upscale ratio above 1, four FNV-1a digests of where the tolerance units look in the G-buffer:
+//   [0] light_gbuffer_index (the light passes' and k_spatial's texel of the pixel),
+//   [1] denoise_deferred_coords (k_demodulation / k_denoise),
+//   [2] previous_pixel, exclusive and inclusive, for velocity 0 and for probe_velocity: the index, or ~0 when rejected,
+//   [3] for both tables, each neighbour's render pixel, the texel of each neighbour inside the frame and of each of its depth-march
+//       taps, as k_spatial computes them.
+__global__ void k_deferred_digest(const __grid_constant__ hkd::KParams P, const __grid_constant__ ProbeTable T16,
+                                  const __grid_constant__ ProbeTable T8, uint32_t frame, uint32_t* out) {
+    const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int RW = P.band.RW, RH = P.band.RH;
+    if (p >= (size_t)RW * RH) return;
+    const int x = (int)(p % (size_t)RW), y = (int)(p / (size_t)RW);
+    const vec2 uv = hkd::render_uv(P, x, y);
+    uint32_t d[4] = {2166136261u, 2166136261u, 2166136261u, 2166136261u};
+
+    size_t g = hkd::light_gbuffer_index(P, x, y, p);
+    d[0] = fnv(fnv(d[0], (uint32_t)(g % (size_t)P.band.AW)), (uint32_t)(g / (size_t)P.band.AW));
+    int dx, dy;
+    hkd::denoise_deferred_coords(P, uv, x, y, dx, dy);
+    d[1] = fnv(fnv(d[1], (uint32_t)dx), (uint32_t)dy);
+    const vec2 velocities[2] = {v2(0.0f, 0.0f), probe_velocity((uint32_t)p, frame)};
+    for (int v = 0; v < 2; ++v) {
+        const vec2 previous_uv = hkd::jittered_deferred_uv(P, uv, 0.25f) - velocities[v];      // as the light passes and k_spatial
+        for (int inclusive = 0; inclusive < 2; ++inclusive) {
+            size_t pidx;
+            d[2] = fnv(d[2], hkd::previous_pixel(P, previous_uv, inclusive != 0, pidx) ? (uint32_t)pidx : 0xFFFFFFFFu);
+        }
+    }
+
+    const float rotation = probe_rotation((uint32_t)p, frame);
+    const vec2 march_uv = hkd::spatial_pixel_uv(x, y, (float)RW, (float)RH);
+    for (int t = 0; t < 2; ++t) {
+        const ProbeTable& T = t == 0 ? T16 : T8;
+        const uint32_t count = t == 0 ? 16u : 8u;
+        for (uint32_t i = 1u; i <= count; ++i) {
+            const vec2 offset = hkd::spatial_offset(T.phase[i], T.radius[i], rotation, P.random_frame);
+            int sx, sy;
+            hkd::spatial_neighbour_pixel(offset, x, y, sx, sy);
+            d[3] = fnv(fnv(d[3], (uint32_t)sx), (uint32_t)sy);
+            if (sx < 0 || sy < 0 || sx >= RW || sy >= RH) continue;
+            g = hkd::light_gbuffer_index(P, sx, sy, hkd::render_index(P.band, sx, sy));
+            d[3] = fnv(fnv(d[3], (uint32_t)(g % (size_t)P.band.AW)), (uint32_t)(g / (size_t)P.band.AW));
+            const vec2 unit = hkd::spatial_march_unit(offset);
+            for (uint32_t j = 1u; j <= T.tap_count[i]; ++j) {
+                int tx, ty;
+                hkd::jittered_deferred_coords(P, hkd::spatial_tap_uv(march_uv, unit, T.tap_dist[i][j - 1u], (float)RW, (float)RH, P.inv_rw,
+                                                                     P.inv_rh), tx, ty);
+                d[3] = fnv(fnv(d[3], (uint32_t)tx), (uint32_t)ty);
+            }
+        }
+    }
+    for (int k = 0; k < 4; ++k) out[4 * p + k] = d[k];
+}
+
+// context.cu, "per-neighbour constants of spatial_reuse"
+static ProbeTable probe_table(uint32_t count, float range) {
+    ProbeTable T = {};
+    for (uint32_t i = 1; i <= count; ++i) {
+        T.phase[i] = (float)i * GOLDEN_RATIO;
+        const float rad = sqrtf((float)i / (float)count) * range;
+        T.radius[i] = rad;
+        const float tap_interval = fmax_(1.0f, rad / 5.0f);
+        const uint32_t tap_count = f32_to_u32(rad / tap_interval);
+        T.tap_count[i] = tap_count > 6u ? 6u : tap_count;
+        for (uint32_t j = 1; j <= T.tap_count[i]; ++j) T.tap_dist[i][j - 1] = (float)j * tap_interval;
+    }
+    return T;
+}
+
 extern "C" {
 
 // Device pointers; `n` inputs of probe_words(fn) words each, n results of as many words as that gives.  Returns the CUDA error code
@@ -182,18 +260,33 @@ int probe_batch(int fn, const uint32_t* in, uint32_t first, uint32_t* out, size_
 }
 
 int probe_spatial_digest(uint32_t count, float range, int w, int h, uint32_t frame, uint32_t* out) {
-    ProbeTable T = {};
-    for (uint32_t i = 1; i <= count; ++i) {      // context.cu, "per-neighbour constants of spatial_reuse"
-        T.phase[i] = (float)i * GOLDEN_RATIO;
-        const float rad = sqrtf((float)i / (float)count) * range;
-        T.radius[i] = rad;
-        const float tap_interval = fmax_(1.0f, rad / 5.0f);
-        const uint32_t tap_count = f32_to_u32(rad / tap_interval);
-        T.tap_count[i] = tap_count > 6u ? 6u : tap_count;
-        for (uint32_t j = 1; j <= T.tap_count[i]; ++j) T.tap_dist[i][j - 1] = (float)j * tap_interval;
-    }
+    const ProbeTable T = probe_table(count, range);
     const size_t n = (size_t)w * h;
     k_spatial_digest<<<(unsigned)((n + 255) / 256), 256>>>(T, count, w, h, frame, random_float(frame), 1.0f / (float)w, 1.0f / (float)h, out);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    return (int)e;
+}
+
+// A w x h full-frame context at upscale ratio `ratio` in (1, 2], frame `frame`: the KParams fields the pixel mapping reads, derived as
+// context.cu's make_params derives them.  `out`: 4 words per render pixel (k_deferred_digest), RW x RH = ceil(size / ratio) pixels
+int probe_deferred_digest(int w, int h, float ratio, uint32_t frame, uint32_t* out) {
+    hkd::KParams P;
+    memset(&P, 0, sizeof(P));
+    P.band.W = w; P.band.H = h;
+    P.band.ax0 = 0; P.band.ax1 = w; P.band.a0 = 0; P.band.a1 = h;
+    P.band.AW = hkd::hk_plane_pitch(w);
+    const float scale = 1.0f / ratio;
+    P.band.RW = (int)ceilf(scale * (float)w); P.band.RH = (int)ceilf(scale * (float)h); P.band.RS = P.band.RW;
+    P.band.cx0 = 0; P.band.cx1 = P.band.RW; P.band.r0 = 0; P.band.r1 = P.band.RH;
+    P.in.frame.number = frame; P.in.frame.upscale_ratio = ratio;
+    P.ratio1 = 0;
+    P.jitter_sign = ((frame & 1u) == 0u) ? -1.0f : 1.0f;
+    P.ratio_m1 = ratio - 1.0f;
+    P.inv_rw = 1.0f / (float)P.band.RW; P.inv_rh = 1.0f / (float)P.band.RH;
+    P.random_frame = random_float(frame);
+    const size_t n = (size_t)P.band.RW * P.band.RH;
+    k_deferred_digest<<<(unsigned)((n + 255) / 256), 256>>>(P, probe_table(16u, 20.0f), probe_table(8u, 10.0f), frame, out);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     return (int)e;

@@ -4,8 +4,8 @@ The parity suite checks the claim "device == oracle because both compile hk_math
 compiles the kernels for the host, so neither ever runs the `__CUDA_ARCH__` branches of the header on inputs the test frames do
 not happen to produce.  tests/cuda/math_probe.cu runs every primitive over an input array on the device, compiled once with the
 flags of the units that trace rays ("exact") and once with those of the tolerance units ("fast", build.py FAST_FLAGS);
-the oracle's hko_math_batch / hko_math_batch_range / hko_spatial_digest run the same inputs on the host.  Every comparison is of
-bits, in chunks of 2^26 values, on the device; a failure names the count and the first differing inputs."""
+the oracle's hko_math_batch / hko_math_batch_range / hko_spatial_digest / hko_deferred_digest run the same inputs on the host.
+Every comparison is of bits, in chunks of 2^26 values, on the device; a failure names the count and the first differing inputs."""
 import ctypes as C
 import math
 
@@ -44,6 +44,8 @@ def probe():
         lib.probe_batch.restype, lib.probe_batch.argtypes = C.c_int, [C.c_int, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t]
         lib.probe_spatial_digest.restype = C.c_int
         lib.probe_spatial_digest.argtypes = [C.c_uint32, C.c_float, C.c_int, C.c_int, C.c_uint32, C.c_void_p]
+        lib.probe_deferred_digest.restype = C.c_int
+        lib.probe_deferred_digest.argtypes = [C.c_int, C.c_int, C.c_float, C.c_uint32, C.c_void_p]
         libs[flavor] = lib
     try:    # an OpenMP team of the machine's size under a smaller CPU quota spends its time throttled (oracle.usable_cpus)
         C.CDLL("libgomp.so.1").omp_set_num_threads(oracle.usable_cpus())
@@ -214,6 +216,48 @@ def test_spatial_neighbour_and_march_tap_pixels_match_the_oracle(probe, size):
                 if bad.size:
                     failures.append((f, count, frame, int(bad.size), [(int(p % w), int(p // w)) for p in bad[:4]]))
     assert not failures, f"(flavour, neighbours, frame, pixels, first pixels): {failures}"
+
+
+# 1.3, 1.5, 1.7, 2 and two fixed f32 draws in (1, 2] (numpy default_rng(20261016)).  At 1.5, W / RW is exactly 1.5 for sizes divisible
+# by 3: half the columns and rows land exactly on a texel edge in real arithmetic, so their texel is decided by the last bit of the uv
+UPSCALE_RATIOS = [1.3, 1.5, 1.7, 2.0, 1.3451449, 1.556715]
+DEFERRED_DIGESTS = ["light texel", "denoise texel", "previous pixel", "spatial neighbours and taps"]
+
+
+def render_size(w, h, ratio):
+    """ceil(size / ratio) as context.cu / the oracle compute it in f32"""
+    scale = np.float32(1.0) / np.float32(ratio)
+    return int(np.ceil(scale * np.float32(w))), int(np.ceil(scale * np.float32(h)))
+
+
+@pytest.mark.parametrize("size", [(1920, 1080), (3840, 2160), (192, 108), (131, 67), (127, 63), (90, 50)])
+def test_render_to_gbuffer_texel_mapping_above_ratio_1_matches_the_oracle(probe, size):
+    """Every render pixel at upscale ratios in (1, 2], frames 1-8 (both jitter signs), both flavours: the G-buffer texel the light
+    passes and k_spatial read (light_gbuffer_index), the one the denoise passes read (denoise_deferred_coords), the reprojected
+    pixel (previous_pixel) for velocity 0 and a drawn velocity, and k_spatial's neighbour pixels with the texels of each neighbour and
+    of its depth-march taps (csrc/hk_device.cuh, csrc/hk_spatial_taps.cuh) equal the oracle's (Deferred::jittered_coords / nearest,
+    load_previous, spatial_neighbour, spatial_tap_uv) bit for bit.  An off-by-one there reads another texel's normal, depth,
+    instance and albedo."""
+    torch, libs, orc = probe
+    w, h = size
+    host = np.empty(w * h * 4, np.uint32)
+    dev = torch.empty(w * h * 4, dtype=torch.int32, device="cuda")
+    failures, counts = [], {}
+    for ratio in UPSCALE_RATIOS:
+        rw, rh = render_size(w, h, ratio)
+        n = rw * rh * 4
+        for frame in range(1, 9):
+            orc.hko_deferred_digest(w, h, ratio, frame, host.ctypes.data)
+            for f in ("exact", "fast"):
+                assert libs[f].probe_deferred_digest(w, h, ratio, frame, dev.data_ptr()) == 0
+                bad = (dev[:n].cpu().numpy().view(np.uint32) != host[:n]).reshape(rw * rh, 4)
+                px = np.flatnonzero(bad.any(axis=1))
+                counts[(f, ratio)] = counts.get((f, ratio), 0) + int(px.size)
+                if px.size:
+                    which = {DEFERRED_DIGESTS[k]: int(bad[:, k].sum()) for k in range(4) if bad[:, k].any()}
+                    failures.append((f, ratio, frame, int(px.size), which, [(int(p % rw), int(p // rw)) for p in px[:4]]))
+    print(f"{w}x{h} differing render pixels over frames 1-8 (flavour, ratio):", counts)
+    assert not failures, f"(flavour, ratio, frame, pixels, per digest, first render pixels): {failures[:12]}"
 
 
 def random_words(rng, n, specials):

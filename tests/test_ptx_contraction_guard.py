@@ -2,10 +2,11 @@
 
 build.py compiles kernels_spatial.cu and kernels_post.cu with -fmad=true -prec-div=false -prec-sqrt=false (FAST_FLAGS).  Under
 those flags nvcc fuses a plain a * b + c into one FMA and ptxas may fuse a `mul.f32` / `add.f32` pair that carries no rounding
-modifier.  sincos_, snorm8, pack2x16unorm (include/hk_math.h), pack_reservoir (csrc/hk_device.cuh) and the spatial-reuse pixel
-helpers (csrc/hk_spatial_taps.cuh) feed f32 -> integer conversions, where one rounding step decides a neighbour, a stored normal
-byte or a lifetime, so they write every product and sum as mul_rn / add_rn (.rn in the PTX: never fused) and every quotient and
-square root as div_rn / sqrt_rn / rcp_rn.  This test cross-compiles each of them alone with the tolerance flags and reads the PTX:
+modifier.  sincos_, snorm8, pack2x16unorm (include/hk_math.h), pack_reservoir (csrc/hk_device.cuh), the spatial-reuse pixel
+helpers (csrc/hk_spatial_taps.cuh) and the render pixel -> G-buffer texel mapping above upscale ratio 1 (csrc/hk_device.cuh) feed
+f32 -> integer conversions, where one rounding step decides a neighbour, a texel, a stored normal byte or a lifetime, so they
+write every product and sum as mul_rn / add_rn (.rn in the PTX: never fused) and every quotient and square root as div_rn /
+sqrt_rn / rcp_rn.  This test cross-compiles each of them alone with the tolerance flags and reads the PTX:
   * no f32 mul / add / sub without .rn, no approximate division, square root or reciprocal;
   * exactly as many FMAs as the exact flags give (the explicit fmaf() calls): none was contracted.
 tests/test_gpu_device_math.py checks the same functions bit for bit on the H100; this keeps them from regressing between GPU runs."""
@@ -17,6 +18,9 @@ import pytest
 
 from bevy_hikari_b200 import build as product_build
 
+# a full-frame context above upscale ratio 1, as context.cu's make_params fills the fields the pixel mapping reads
+DEFERRED_PARAMS = ("hkd::KParams P; P.ratio1 = 0; P.band.W = n[0]; P.band.H = n[1]; P.band.RW = n[2]; P.band.RH = n[3]; P.band.RS = n[2]; "
+                   "P.band.AW = n[0]; P.band.ax0 = 0; P.band.a0 = 0; P.jitter_sign = i[0]; P.ratio_m1 = i[1]; ")
 SNIPPETS = {
     "sincos_": "float s, c; hk::sincos_(i[0], &s, &c); o[0] = s; o[1] = c;",
     "snorm8": "u[0] = hk::snorm8(i[0]);",
@@ -30,6 +34,18 @@ SNIPPETS = {
                          "hk::vec2 unit = hkd::spatial_march_unit(hk::v2(i[0], i[1])); int tx, ty; "
                          "hkd::spatial_tap_pixel(hkd::spatial_tap_uv(uv, unit, i[2], i[4], i[5], i[6], i[7]), n[2], n[3], tx, ty); "
                          "u[0] = tx; u[1] = ty;",
+    # render pixel -> G-buffer texel above upscale ratio 1 (csrc/hk_device.cuh): k_spatial, k_demodulation, k_denoise
+    "light_deferred_coords": DEFERRED_PARAMS + "int dx, dy; hkd::light_deferred_coords(P, hkd::render_uv(P, n[4], n[5]), n[4], n[5], dx, dy); "
+                             "u[0] = dx; u[1] = dy;",
+    "denoise_deferred_coords": DEFERRED_PARAMS + "int dx, dy; hkd::denoise_deferred_coords(P, hkd::render_uv(P, n[4], n[5]), n[4], n[5], dx, dy); "
+                               "u[0] = dx; u[1] = dy;",
+    # (the callers' uv - velocity before it is a subtraction of two loaded or correctly rounded values: nothing to contract)
+    "previous_pixel": DEFERRED_PARAMS + "hk::vec2 uv = hkd::jittered_deferred_uv(P, hkd::render_uv(P, n[4], n[5]), 0.25f); size_t pidx = 0; "
+                      "u[0] = hkd::previous_pixel(P, hk::v2(i[2], i[3]), n[6] != 0, pidx); u[1] = (unsigned)pidx; o[0] = uv.x; o[1] = uv.y;",
+    "spatial_deferred_tap": DEFERRED_PARAMS + "hk::vec2 uv = hkd::spatial_pixel_uv(n[4], n[5], (float)n[2], (float)n[3]); "
+                            "hk::vec2 unit = hkd::spatial_march_unit(hk::v2(i[2], i[3])); int tx, ty; "
+                            "hkd::jittered_deferred_coords(P, hkd::spatial_tap_uv(uv, unit, i[4], (float)n[2], (float)n[3], i[5], i[6]), tx, ty); "
+                            "u[0] = tx; u[1] = ty;",
 }
 SOURCE = """#include "hk_device.cuh"
 #include "hk_spatial_taps.cuh"
