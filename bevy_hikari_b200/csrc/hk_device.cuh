@@ -957,6 +957,11 @@ constexpr int TILE_W = 16, TILE_H = 2 * HK_CTA_WARPS, CTA_THREADS = 32 * HK_CTA_
 #ifndef HK_MINB_DIRECT
 #define HK_MINB_DIRECT 8
 #endif
+#ifndef HK_MINB_DIRECT_UNTEXTURED
+#define HK_MINB_DIRECT_UNTEXTURED 5   // k_direct's TEX = false instantiations (untextured scenes).  H100 SXM 700 W, direct + emissive ms
+                                      // on cornell 1080p at 5 / 6 / 7 / 8 CTAs/SM: 0.497 / 0.514 / 0.540 / 0.570; the textured city 4K and
+                                      // scene.rs 1080p frames are 1-2 % slower below 8 (profiles/h100_ab_direct_bounds.json, DESIGN.md 4a-5)
+#endif
 #ifndef HK_MINB_GBUFFER
 #define HK_MINB_GBUFFER 8    // 64 registers instead of the 66-78 an uncapped build takes
 #endif

@@ -201,7 +201,8 @@ __global__ void __launch_bounds__(CTA_THREADS) k_albedo(const __grid_constant__ 
 // traversal, a second TLAS traversal, the reset logic — is not in the kernel (2 of 3 sun frames, 4 of 5 emissive frames at the
 // default intervals).  The generic instantiation decides the same thing at run time; values are identical.
 template <bool EMISSIVE_LIT, bool COUNT, bool TEX = true, bool NOVAL = false, bool WIDE = false>
-__global__ void __launch_bounds__(CTA_THREADS, WIDE ? HK_MINB_DIRECT_WIDE : HK_MINB_DIRECT) k_direct(const __grid_constant__ KParams P) {
+__global__ void __launch_bounds__(CTA_THREADS, WIDE ? HK_MINB_DIRECT_WIDE : (TEX ? HK_MINB_DIRECT : HK_MINB_DIRECT_UNTEXTURED))
+k_direct(const __grid_constant__ KParams P) {
     constexpr int SIGNAL = EMISSIVE_LIT ? 1 : 0;
     constexpr bool RENDER_EMISSIVE = !EMISSIVE_LIT;
     int x, y;
