@@ -74,6 +74,7 @@ struct hk_context {
     uint32_t scene_material_count = 0, scene_asset_node_count = 0, scene_primitive_count = 0, scene_vertex_count = 0, scene_texture_count = 0;
     std::vector<hk_node> host_asset_nodes;                 // copy of the uploaded BLAS records: index validation of later instance updates
     std::vector<uint32_t> host_primitive_vertex_index;     // 3 per primitive (hk_primitive_vertex::index), same purpose
+    std::vector<float> host_primitive_box;                 // 6 per primitive (min xyz, max xyz): what a BLAS leaf's navigator must enclose
     std::set<std::array<uint32_t, 4>> mesh_range_checked;   // hk_mesh_index values whose leaves have been validated
     Planes planes{};
     DeviceScene scene{};
@@ -471,10 +472,12 @@ static cudaError_t upload_into(hk_context* ctx, hk_context::DevBuf& b, const T**
 }
 
 // The 4-wide tree over the instances (the half of upload_wide that every instance update repeats) from the flat TLAS in `nodes`
-// (host memory); the meshes' trees and ctx->wide_mesh_of are those of the last upload_wide.
-static int upload_wide_tlas(hk_context* ctx, const hk_node* nodes, uint32_t node_count, uint32_t instance_count, DeviceScene& d) {
+// (host memory) and the instances' boxes (6 floats each, or null when the navigators carry them by construction); the meshes' trees
+// and ctx->wide_mesh_of are those of the last upload_wide.
+static int upload_wide_tlas(hk_context* ctx, const hk_node* nodes, uint32_t node_count, uint32_t instance_count, const float* instance_box,
+                            DeviceScene& d) {
     d.wide_ready = 0u; d.wide_tlas_root = WIDE_EMPTY;
-    hkw::WideTree tlas = hkw::build_wide(nodes, node_count, instance_count);
+    hkw::WideTree tlas = hkw::build_wide(nodes, node_count, instance_count, instance_box);
     bool ok = tlas.ok && ctx->wide_mesh_of.size() == instance_count;
     uint32_t blas_need = 0;
     std::vector<uint2> entry(instance_count);
@@ -525,9 +528,13 @@ static int upload_wide(hk_context* ctx, const hk_scene_desc* s, DeviceScene& d) 
             uint32_t shapes = 0;
             for (uint32_t r = 0; r < keys[k][1]; ++r)
                 if (flat[r].entry_index >= 0x80000000u) shapes = std::max(shapes, flat[r].entry_index - 0x80000000u + 1u);
-            hkw::WideTree t = hkw::build_wide(flat, keys[k][1], shapes);
+            hkw::WideTree t = hkw::build_wide(flat, keys[k][1], shapes, ctx->host_primitive_box.data() + 6 * (size_t)keys[k][2]);
             meshes[k].ok = t.ok;
             if (!t.ok) continue;
+            if (t.root == WIDE_EMPTY) {      // a mesh without records: WIDE_EMPTY as its entry point would end the whole walk, not
+                t.nodes.assign(1, hkw::empty_node());       // just the instance; a node without children returns to the TLAS
+                t.root = 0;
+            }
             meshes[k].base = (uint32_t)all.size(); meshes[k].root = t.root; meshes[k].need = t.stack_need;
             all.insert(all.end(), t.nodes.begin(), t.nodes.end());
             for (uint32_t sh = 0; sh < shapes; ++sh)
@@ -542,7 +549,10 @@ static int upload_wide(hk_context* ctx, const hk_scene_desc* s, DeviceScene& d) 
         d.wide_primitive_rank = reinterpret_cast<const uint32_t*>(ctx->ibuf[13].p);
     }
     ctx->wide_mesh_of = mesh_of;
-    return upload_wide_tlas(ctx, s->instance_nodes, s->instance_node_count, s->instance_count, d);
+    std::vector<float> instance_box(6 * (size_t)s->instance_count);
+    for (uint32_t i = 0; i < s->instance_count; ++i)
+        for (int c = 0; c < 3; ++c) { instance_box[6 * (size_t)i + c] = s->instances[i].min[c]; instance_box[6 * (size_t)i + 3 + c] = s->instances[i].max[c]; }
+    return upload_wide_tlas(ctx, s->instance_nodes, s->instance_node_count, s->instance_count, instance_box.data(), d);
 }
 
 // Validation + upload of the per-frame half of the scene (instances, TLAS, emissives, emissive BVH, alias tables,
@@ -728,6 +738,14 @@ int hk_scene_upload(hk_context* ctx, const hk_scene_desc* s) {
     ctx->host_primitive_vertex_index.resize(3 * (size_t)s->primitive_count);
     for (uint32_t i = 0; i < s->primitive_count; ++i)
         for (int c = 0; c < 3; ++c) ctx->host_primitive_vertex_index[3 * (size_t)i + c] = s->primitives[i].vertices[c].index;
+    ctx->host_primitive_box.resize(6 * (size_t)s->primitive_count);
+    for (uint32_t i = 0; i < s->primitive_count; ++i) {
+        const hk_primitive& p = s->primitives[i];
+        for (int c = 0; c < 3; ++c) {
+            ctx->host_primitive_box[6 * (size_t)i + c] = fminf(p.vertices[0].position[c], fminf(p.vertices[1].position[c], p.vertices[2].position[c]));
+            ctx->host_primitive_box[6 * (size_t)i + 3 + c] = fmaxf(p.vertices[0].position[c], fmaxf(p.vertices[1].position[c], p.vertices[2].position[c]));
+        }
+    }
     // primitives index vertices relative to their mesh's vertex base: the largest index of each mesh is checked per instance
     // below through mesh.vertex + index < vertex_count for the primitives of its leaves
     DeviceScene d{};
@@ -876,7 +894,7 @@ int hk_scene_update_transforms(hk_context* ctx, const float* models, const float
         std::vector<hk_node> nodes(tlas_records);
         HK_CUDA(cudaMemcpyAsync(nodes.data(), ctx->ibuf[2].p, sizeof(hk_node) * (size_t)tlas_records, cudaMemcpyDeviceToHost, ctx->stream));
         HK_CUDA(cudaStreamSynchronize(ctx->stream));
-        int rc = upload_wide_tlas(ctx, nodes.data(), tlas_records, n, d);
+        int rc = upload_wide_tlas(ctx, nodes.data(), tlas_records, n, nullptr, d);     // leaf navigators = instance boxes, as built
         if (rc != HK_OK) return rc;
     }
     ctx->scene = d;

@@ -6,7 +6,14 @@
 // parsed back, collapsed to at most four children per node by opening the child with the largest surface area first, and written
 // pre-order.  What the walk needs besides the nodes: the position of every shape's leaf in the flat array (its rank: the reference's
 // strict '<' keeps the FIRST of two equidistant hits in that order, light.wgsl:416,470) and the deepest stack the tree can ask for.
-// A flat array that does not have this shape (a foreign BVH) yields ok = false: the context then keeps the exact-order walk.
+// Foreign flat arrays in the same skip-link layout are accepted as long as the derived tree walks exactly like the flat one: any
+// arity from 1 up, runs of up to four branches below a navigator and at the top level, navigator boxes larger than what they hold.
+// ok = false — the context then keeps the exact-order walk — for an array that is not in this layout (links that do not nest, a leaf
+// named twice, a leaf that names no shape), for a node that still has more than four branches after collapsing (a 4-wide node cannot
+// hold them; bvh 0.7.1 writes two) and for a navigator box that does not enclose the boxes below it (its children's navigator boxes,
+// or the shape's own box at a leaf).  Such a box culls hits it does not enclose, and whether it does depends on the best hit found so
+// far, i.e. on the order of the walk; the 4-wide walk also never tests the boxes of the binary levels it collapses.  An empty array
+// is ok with root = EMPTY: the context gives such a mesh a node without children (empty_node) to enter.
 #pragma once
 #include <stdint.h>
 
@@ -28,6 +35,17 @@ struct WideTree {
     std::vector<uint32_t> node_need;       // (internal) per wide node
 };
 
+// a node without children: the walk tests nothing in it and pops
+inline hkd::hk_wide_node empty_node() {
+    hkd::hk_wide_node n;
+    const float inf = std::numeric_limits<float>::infinity();
+    for (int c = 0; c < 4; ++c) {
+        n.lo_x[c] = n.lo_y[c] = n.lo_z[c] = inf; n.hi_x[c] = n.hi_y[c] = n.hi_z[c] = -inf;
+        n.child[c] = hkd::WIDE_EMPTY; n.pad[c] = 0u;
+    }
+    return n;
+}
+
 namespace detail {
 
 struct BNode {
@@ -37,11 +55,18 @@ struct BNode {
     std::vector<uint32_t> kids;
 };
 
+inline bool encloses(const float* lo, const float* hi, const float* inner_lo, const float* inner_hi) {
+    for (int k = 0; k < 3; ++k)
+        if (!(lo[k] <= inner_lo[k] && inner_hi[k] <= hi[k])) return false;      // false for NaN too
+    return true;
+}
+
 struct Parser {
     const hk_node* flat;
     uint32_t count;
     std::vector<BNode>& out;
     std::vector<uint32_t>& rank;
+    const float* shape_box;        // 6 per shape (min xyz, max xyz), or null when the leaves' boxes are the shapes' by construction
     uint32_t leaves = 0;
     bool ok = true;
 
@@ -60,15 +85,19 @@ struct Parser {
                 if (nav.exit_index != i + 2 || first.exit_index != i + 2 || shape >= rank.size() || rank[shape] != 0xFFFFFFFFu) { ok = false; break; }
                 b.leaf = true; b.shape = shape;
                 rank[shape] = leaves++;
+                if (shape_box && !encloses(b.lo, b.hi, shape_box + 6 * (size_t)shape, shape_box + 6 * (size_t)shape + 3)) { ok = false; break; }
             } else {
                 b.leaf = false; b.shape = 0;
                 b.kids = range(i + 1, nav.exit_index, depth + 1);
                 if (b.kids.empty()) ok = false;
+                for (uint32_t kid : b.kids) ok = ok && encloses(b.lo, b.hi, out[kid].lo, out[kid].hi);
             }
             out.push_back(std::move(b));
             kids.push_back((uint32_t)out.size() - 1);
             i = nav.exit_index;
         }
+        // a run of more than four branches: no child of the run can be opened to make room, so a 4-wide node would drop some
+        if (kids.size() > 4) ok = false;
         return kids;
     }
 };
@@ -97,12 +126,7 @@ inline uint32_t emit(const std::vector<BNode>& b, std::vector<uint32_t> kids, Wi
     const uint32_t index = (uint32_t)t.nodes.size();
     t.nodes.emplace_back();
     t.node_need.push_back(0);
-    hkd::hk_wide_node n;
-    const float inf = std::numeric_limits<float>::infinity();
-    for (int c = 0; c < 4; ++c) {
-        n.lo_x[c] = n.lo_y[c] = n.lo_z[c] = inf; n.hi_x[c] = n.hi_y[c] = n.hi_z[c] = -inf;
-        n.child[c] = hkd::WIDE_EMPTY; n.pad[c] = 0u;
-    }
+    hkd::hk_wide_node n = empty_node();
     uint32_t need = 0;
     const uint32_t k = (uint32_t)std::min<size_t>(kids.size(), 4);
     for (uint32_t c = 0; c < k; ++c) {
@@ -126,8 +150,9 @@ inline uint32_t emit(const std::vector<BNode>& b, std::vector<uint32_t> kids, Wi
 
 }  // namespace detail
 
-// `shape_count`: number of shapes the leaves may name (triangles of the mesh / instances of the scene)
-inline WideTree build_wide(const hk_node* flat, uint32_t count, uint32_t shape_count) {
+// `shape_count`: number of shapes the leaves may name (triangles of the mesh / instances of the scene); `shape_box`: their boxes, 6
+// floats each (min xyz, max xyz), which every leaf's navigator box must enclose — null where the caller wrote those boxes itself
+inline WideTree build_wide(const hk_node* flat, uint32_t count, uint32_t shape_count, const float* shape_box) {
     WideTree t;
     t.rank.assign(shape_count, 0xFFFFFFFFu);
     if (count == 0) { t.ok = true; return t; }
@@ -140,11 +165,9 @@ inline WideTree build_wide(const hk_node* flat, uint32_t count, uint32_t shape_c
     }
     std::vector<detail::BNode> b;
     b.reserve(count);
-    detail::Parser p{flat, count, b, t.rank};
+    detail::Parser p{flat, count, b, t.rank, shape_box};
     std::vector<uint32_t> top = p.range(0, count, 0);
     if (!p.ok || top.empty()) return t;
-    // more than four branches at the top level would need a synthetic node; bvh 0.7.1 writes exactly two
-    if (top.size() > 4) return t;
     t.root = detail::emit(b, top, t);
     t.stack_need = t.node_need[t.root];
     t.ok = true;

@@ -311,9 +311,13 @@ int hk_set_profiling_kernel(hk_context* ctx, int kernel);
  * scene's size (A/B runs and the mode's tests).  Box and triangle tests, their arithmetic and the tie rule (first in array order
  * among equidistant hits) are the reference's, so G-buffer ids, hit distances and every image are the exact walk's except for rays
  * whose two nearest hits tie within the rounding of a box test; under 3 the any-hit OCCLUDER a shadow ray reports (stored with
- * zero-radiance samples, read by no image) depends on the order and differs.  Default 0 in libhikari_b200_exact.so.  A scene whose
- * flat arrays are not bvh 0.7.1's flatten_custom layout, or whose trees could overflow the walk's stack, silently keeps the
- * reference's walk (hk_frame_stats.wide_traversal: bit 0 = primary rays, bit 1 = light passes). */
+ * zero-radiance samples, read by no image) depends on the order and differs.  Default 0 in libhikari_b200_exact.so.  Flat arrays
+ * need not come from bvh 0.7.1: any tree in the same skip-link layout (navigator, then a leaf record or more branches) is walked,
+ * including meshes without records and navigator boxes larger than what they hold.  A scene silently keeps the reference's walk
+ * when one of its flat arrays is not in that layout, names a shape in two leaves, has a run of more than four branches below a
+ * navigator or at the top level, or has a navigator box that does not enclose the boxes below it (its children's navigators, or
+ * the shape's own box at a leaf), or when its trees could overflow the walk's stack (hk_frame_stats.wide_traversal: bit 0 =
+ * primary rays, bit 1 = light passes). */
 enum { HK_TUNE_POOLED_INDIRECT = 1, HK_TUNE_TILED_SPATIAL = 2, HK_TUNE_TILED_DENOISE = 3, HK_TUNE_WIDE_TRAVERSAL = 4 };
 int hk_set_tuning(hk_context* ctx, int key, int value);
 int hk_set_keep_intermediates(hk_context* ctx, int keep);   /* 1: hk_render_frame also writes HK_OUT_DENOISED_* */

@@ -15,8 +15,8 @@ from tests.conftest import ROOT
 
 FILES = ["tests/test_gpu_parity.py", "tests/test_gpu_variants.py", "tests/test_gpu_upscale.py", "tests/test_gpu_dynamic.py",
          "tests/test_gpu_frame_assembly.py", "tests/test_gpu_zz_fsr.py", "tests/test_gpu_zz_examples.py", "tests/test_gpu_zz_halo.py",
-         "tests/test_gpu_wide_traversal.py", "tests/test_gpu_scene_update.py", "tests/test_gpu_wgsl_golden.py",
-         "tests/test_gpu_zzz_wgsl_late_cases.py", "tests/test_gpu_zzz_late_regressions.py"]
+         "tests/test_gpu_wide_traversal.py", "tests/test_gpu_wide_foreign_bvh.py", "tests/test_gpu_scene_update.py",
+         "tests/test_gpu_wgsl_golden.py", "tests/test_gpu_zzz_wgsl_late_cases.py", "tests/test_gpu_zzz_late_regressions.py"]
 # the reverse order runs single-threaded: the files whose kernels have something an order could change (scatter claims / resolve,
 # cooperative tiles and pools, the level-synchronous BVH build, halo copies), not the long fixture sequences once more
 REVERSE_FILES = ["tests/test_gpu_parity.py", "tests/test_gpu_upscale.py", "tests/test_gpu_dynamic.py", "tests/test_gpu_zz_halo.py",
