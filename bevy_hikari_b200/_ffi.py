@@ -65,6 +65,13 @@ SYMBOLS = {
     "hk_scene_update_transforms": (_I, [_P, _P, _P, _P, _U32]),
     "hk_scene_readback": (_I, [_P, _I, _P, _SZ]),
     "hk_scene_buffer_bytes": (_I, [_P, _I, C.POINTER(_SZ)]),
+    "hk_shared_scene_create": (_I, [C.POINTER(_P), _I, _P]),
+    "hk_shared_scene_destroy": (None, [_P]),
+    "hk_shared_scene_upload": (_I, [_P, C.POINTER(L.SceneDesc)]),
+    "hk_shared_scene_update_instances": (_I, [_P, C.POINTER(L.SceneDesc)]),
+    "hk_shared_scene_update_transforms": (_I, [_P, _P, _P, _P, _U32]),
+    "hk_shared_scene_last_error": (C.c_char_p, [_P]),
+    "hk_context_attach_scene": (_I, [_P, _P]),
     "hk_sync": (_I, [_P]),
     "hk_trace_rays": (_I, [_P, _P, _SZ, _P]),
     "hk_set_profiling": (_I, [_P, _I, _I]),
@@ -114,12 +121,20 @@ SYMBOLS = {
     "hikari_plugin_frame_counter": (_U64, [_P]),
     "hikari_plugin_set_frame_counter": (None, [_P, _U64]),
     "hikari_plugin_set_temporal_upscalers": (None, [_P, _I]),
+    "hikari_shared_scene_create": (_P, []),
+    "hikari_shared_scene_destroy": (None, [_P]),
+    "hikari_shared_scene_build": (_I, [_P, _I, _P]),
+    "hikari_shared_scene_upload": (_I, [_P, _P]),
+    "hikari_shared_scene_update_instances": (_I, [_P, _P]),
+    "hikari_shared_scene_update_transforms": (_I, [_P, _P, C.POINTER(_I)]),
+    "hikari_shared_scene_handle": (_P, [_P]),
+    "hikari_plugin_attach_scene": (_I, [_P, _P]),
 }
 
 _lib = None
 _host_lib = None
 # symbols of include/hikari_host.h that live in libhikari_host.so (no CUDA behind them)
-HOST_ONLY = [n for n in SYMBOLS if n.startswith("hikari_") and not n.startswith("hikari_plugin_")]
+HOST_ONLY = [n for n in SYMBOLS if n.startswith("hikari_") and not n.startswith(("hikari_plugin_", "hikari_shared_scene_"))]
 
 
 def host_lib():

@@ -48,13 +48,19 @@ struct hk_halo_peer {   // a neighbour tile of another process, mapped through C
     void* mapped[44];
 };
 
-struct hk_context {
+// The scene a context renders: meshes, BLAS nodes, materials, textures, the per-frame instance half, the 4-wide trees and the host
+// copies that validate later updates.  The reference keeps one such set for the whole render world (MeshMaterialBindGroup,
+// mesh_material/mod.rs:677-681) and every camera's LightNode binds it (light.rs:641-642); here several contexts attach to one scene
+// (hk_shared_scene_create), or hk_scene_upload gives a context a private one on the context's own stream.
+struct hk_shared_scene {
     int device = 0;
-    cudaStream_t stream = nullptr;
+    cudaStream_t stream = nullptr;         // uploads and updates run here
     bool own_stream = false;
-    Band band{};
-    size_t band_pixels = 0, owned_pixels = 0;
-    std::vector<void*> allocations;        // per-pixel planes
+    bool handle = true;                    // the creator's hk_shared_scene handle is alive (a private scene has none)
+    hk_context* owner = nullptr;           // private scene: the one context whose hk_scene_upload / hk_scene_update_* write it
+    std::vector<hk_context*> attached;     // the scene is freed when the handle is gone and the last context detached
+    uint64_t version = 0;                  // bumped by every upload / update
+    cudaEvent_t ev_ready = nullptr;        // recorded after an update when an attached context runs on another stream
     std::vector<void*> scene_allocations;  // scene buffers: meshes, BLAS nodes, materials, textures
     struct DevBuf { void* p = nullptr; size_t cap = 0; } ibuf[20];  // scene buffers rewritten by hk_scene_update_instances (grow-only);
                                                                     // 14-19: staging + scratch of hk_scene_update_transforms
@@ -69,6 +75,7 @@ struct hk_context {
     std::vector<std::array<uint32_t, 3>> wide_mesh_keys;    // (node_offset, node_count, primitive) in first-use order
     std::vector<WideMesh> wide_meshes;                      // parallel to wide_mesh_keys
     uint32_t wide_blas_node_count = 0;
+    uint32_t wide_tlas_node_count = 0;
     uint32_t wide_stack_need = 0;
     bool mesh_boxes_match = false;         // BLAS half of DeviceScene::leaf_boxes_match
     uint32_t scene_material_count = 0, scene_asset_node_count = 0, scene_primitive_count = 0, scene_vertex_count = 0, scene_texture_count = 0;
@@ -76,9 +83,26 @@ struct hk_context {
     std::vector<uint32_t> host_primitive_vertex_index;     // 3 per primitive (hk_primitive_vertex::index), same purpose
     std::vector<float> host_primitive_box;                 // 6 per primitive (min xyz, max xyz): what a BLAS leaf's navigator must enclose
     std::set<std::array<uint32_t, 4>> mesh_range_checked;   // hk_mesh_index values whose leaves have been validated
-    Planes planes{};
     DeviceScene scene{};
-    bool scene_ready = false, noise_ready = false;
+    bool ready = false;
+    std::string error;
+};
+
+struct hk_context {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    bool own_stream = false;
+    Band band{};
+    size_t band_pixels = 0, owned_pixels = 0;
+    std::vector<void*> allocations;        // per-pixel planes
+    // the scene this context renders (hk_context_attach_scene, or the private one of hk_scene_upload); stream ordering against it
+    // only when it runs on another stream: the version of it this stream has waited for, and "the last frame is done reading it"
+    hk_shared_scene* sc = nullptr;
+    uint64_t scene_seen = 0;
+    cudaEvent_t ev_released = nullptr;
+    bool released_recorded = false;
+    Planes planes{};
+    bool noise_ready = false;
     bool planes_ready = false;         // allocate_planes completed: every pointer of `planes` is valid
     // TMA descriptors of kc_spatial's tiles (hk_tile.cuh): [0] indirect (radius 20, box 56), [1] emissive (radius 10, box 36);
     // q3 maps per buffer parity: the temporal reservoir the spatial pass reuses is reservoir[base + 1 - (frame.number & 1)]
@@ -101,7 +125,6 @@ struct hk_context {
     bool tiled_spatial = true;                        // hk_set_tuning(HK_TUNE_TILED_SPATIAL): kc_spatial (TMA tiles) vs k_spatial (gathers)
     int wide_traversal = 0;                           // hk_set_tuning(HK_TUNE_WIDE_TRAVERSAL): 0 = the reference's fixed-order walk, 1 = primary rays
                                                       // walk the 4-wide trees (scenes deep enough to gain), 3 = every ray does
-    uint32_t wide_tlas_node_count = 0;
     // pipelined read-back (hk_readback_async): copy stream + "frame submitted" / "copy landed" events
     cudaStream_t copy_stream = nullptr;
     cudaEvent_t ev_submitted = nullptr, ev_copied = nullptr;
@@ -134,13 +157,23 @@ static int set_error(hk_context* c, int code, const std::string& msg) {
     if (c) c->error = msg; else g_create_error = msg;
     return code;
 }
-#define HK_CUDA(call)                                                                                      \
+static int set_error(hk_shared_scene* s, int code, const std::string& msg) {
+    if (s) s->error = msg; else g_create_error = msg;
+    return code;
+}
+static int set_error(std::nullptr_t, int code, const std::string& msg) {   // a failed create: hk_last_error(NULL)
+    g_create_error = msg;
+    return code;
+}
+#define HK_CUDA_ON(obj, call)                                                                              \
     do {                                                                                                   \
         cudaError_t e__ = (call);                                                                          \
         if (e__ != cudaSuccess)                                                                            \
-            return set_error(ctx, e__ == cudaErrorMemoryAllocation ? HK_ERR_OUT_OF_MEMORY : HK_ERR_CUDA,   \
+            return set_error(obj, e__ == cudaErrorMemoryAllocation ? HK_ERR_OUT_OF_MEMORY : HK_ERR_CUDA,   \
                              std::string(#call) + ": " + cudaGetErrorString(e__));                         \
     } while (0)
+#define HK_CUDA(call) HK_CUDA_ON(ctx, call)     // in functions of a context
+#define HK_SCUDA(call) HK_CUDA_ON(sc, call)     // in functions of a scene
 
 template <class T>
 static cudaError_t alloc_plane(hk_context* ctx, T** out, size_t count, std::vector<void*>& list) {
@@ -157,6 +190,82 @@ static void free_list(std::vector<void*>& list) {
     for (void* p : list) cudaFree(p);
     list.clear();
 }
+
+// ------------------------------------------------------------------------------------------------ scene ownership + ordering
+// A scene and the contexts attached to it may run on different streams.  Then every scene update first makes the scene's stream
+// wait for each such context's "released" event (recorded after the last launch of a frame entry point that reads the scene),
+// rewrites its buffers, records "ready" and bumps the version; a context's stream waits for "ready" before its first launch that
+// reads a new version.  When a context runs on the scene's own stream — always the case for a private scene — stream order already
+// says all of this and no event is recorded or waited for.
+static bool scene_cross(const hk_shared_scene* sc) {      // some attached context runs on another stream
+    for (const hk_context* c : sc->attached)
+        if (c->stream != sc->stream) return true;
+    return false;
+}
+static void scene_begin_write(hk_shared_scene* sc) {
+    for (hk_context* c : sc->attached)
+        if (c->stream != sc->stream && c->released_recorded) cudaStreamWaitEvent(sc->stream, c->ev_released, 0);
+}
+static void scene_end_write(hk_shared_scene* sc) {
+    sc->version += 1;
+    if (scene_cross(sc) && (sc->ev_ready || cudaEventCreateWithFlags(&sc->ev_ready, cudaEventDisableTiming) == cudaSuccess))
+        cudaEventRecord(sc->ev_ready, sc->stream);
+}
+// before a scene buffer is freed: the released events the scene's stream waits for have completed (grow-only re-allocations and
+// full re-uploads are rare; on the scene's own stream cudaFree is ordered as it always was)
+static void scene_before_free(hk_shared_scene* sc) {
+    if (scene_cross(sc)) cudaStreamSynchronize(sc->stream);
+}
+static void scene_free(hk_shared_scene* sc) {
+    cudaSetDevice(sc->device);
+    if (sc->stream) cudaStreamSynchronize(sc->stream);
+    free_list(sc->scene_allocations);
+    for (auto& b : sc->ibuf) { if (b.p) cudaFree(b.p); b.p = nullptr; b.cap = 0; }
+    for (auto& b : sc->pin) { if (b.p) cudaFreeHost(b.p); if (b.ev) cudaEventDestroy(b.ev); b = hk_shared_scene::PinBuf(); }
+    if (sc->ev_ready) cudaEventDestroy(sc->ev_ready);
+    if (sc->own_stream && sc->stream) cudaStreamDestroy(sc->stream);
+    delete sc;
+}
+static int attach_scene(hk_context* ctx, hk_shared_scene* sc) {
+    if (sc->stream != ctx->stream) {      // frames of this context wait for whatever the scene's stream has queued so far
+        if (!ctx->ev_released) HK_CUDA(cudaEventCreateWithFlags(&ctx->ev_released, cudaEventDisableTiming));
+        if (!sc->ev_ready) HK_CUDA(cudaEventCreateWithFlags(&sc->ev_ready, cudaEventDisableTiming));
+        HK_CUDA(cudaEventRecord(sc->ev_ready, sc->stream));
+        HK_CUDA(cudaStreamWaitEvent(ctx->stream, sc->ev_ready, 0));
+    }
+    sc->attached.push_back(ctx);
+    ctx->sc = sc;
+    ctx->scene_seen = sc->version;
+    ctx->released_recorded = false;
+    return HK_OK;
+}
+static void detach_scene(hk_context* ctx) {
+    hk_shared_scene* sc = ctx->sc;
+    if (!sc) return;
+    if (sc->stream != ctx->stream && ctx->released_recorded) cudaStreamWaitEvent(sc->stream, ctx->ev_released, 0);
+    sc->attached.erase(std::remove(sc->attached.begin(), sc->attached.end(), ctx), sc->attached.end());
+    if (sc->owner == ctx) sc->owner = nullptr;
+    ctx->sc = nullptr;
+    ctx->released_recorded = false;
+    if (!sc->handle && sc->attached.empty()) scene_free(sc);
+}
+static bool scene_ready(const hk_context* ctx) { return ctx->sc && ctx->sc->ready; }
+// Brackets the launches of a frame entry point that read the scene: waits for a new version first, records "released" at the end.
+struct SceneUse {
+    hk_context* c;
+    explicit SceneUse(hk_context* ctx) : c(ctx) {
+        hk_shared_scene* sc = c->sc;
+        if (sc->stream != c->stream && c->scene_seen != sc->version) {
+            if (sc->ev_ready) cudaStreamWaitEvent(c->stream, sc->ev_ready, 0);
+            c->scene_seen = sc->version;
+        }
+    }
+    ~SceneUse() {
+        if (c->sc->stream == c->stream) return;
+        cudaEventRecord(c->ev_released, c->stream);
+        c->released_recorded = true;
+    }
+};
 
 // One TMA descriptor: a 2-D tensor of `width` x `height` elements of `elem_bytes` (row pitch `pitch_bytes`) read in boxes of
 // box_w x box_h elements, no swizzle, zero fill outside.  Encoded by the driver (cuTensorMapEncodeTiled, looked up through the
@@ -392,9 +501,8 @@ void hk_context_destroy(hk_context* ctx) {
     if (ctx->ev_submitted) cudaEventDestroy(ctx->ev_submitted);
     if (ctx->ev_copied) cudaEventDestroy(ctx->ev_copied);
     free_list(ctx->allocations);
-    free_list(ctx->scene_allocations);
-    for (auto& b : ctx->ibuf) { if (b.p) cudaFree(b.p); b.p = nullptr; b.cap = 0; }
-    for (auto& b : ctx->pin) { if (b.p) cudaFreeHost(b.p); if (b.ev) cudaEventDestroy(b.ev); b = hk_context::PinBuf(); }
+    detach_scene(ctx);                     // frees a private scene, and a shared one whose handle and other contexts are gone
+    if (ctx->ev_released) cudaEventDestroy(ctx->ev_released);
     if (ctx->noise) cudaFree(ctx->noise);
     if (ctx->counters) cudaFree(ctx->counters);
     if (ctx->spatial_tables) cudaFree(ctx->spatial_tables);
@@ -438,15 +546,15 @@ int hk_reset_temporal_state(hk_context* ctx) {
 }  // extern "C"
 
 template <class T>
-static cudaError_t upload(hk_context* ctx, const T** dst, const T* src, uint32_t count) {
+static cudaError_t upload(hk_shared_scene* sc, const T** dst, const T* src, uint32_t count) {
     void* p = nullptr;
     size_t bytes = (size_t)count * sizeof(T);
     cudaError_t e = cudaMalloc(&p, bytes + 64);   // +64: 16-byte vector loads at the tail stay in bounds
     if (e != cudaSuccess) return e;
-    ctx->scene_allocations.push_back(p);
-    e = cudaMemsetAsync(p, 0, bytes + 64, ctx->stream);
+    sc->scene_allocations.push_back(p);
+    e = cudaMemsetAsync(p, 0, bytes + 64, sc->stream);
     if (e != cudaSuccess) return e;
-    if (bytes) e = cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
+    if (bytes) e = cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, sc->stream);
     *dst = reinterpret_cast<const T*>(p);
     return e;
 }
@@ -454,48 +562,48 @@ static cudaError_t upload(hk_context* ctx, const T** dst, const T* src, uint32_t
 
 // copy into a grow-only device buffer (per-frame updates must not pay cudaMalloc/cudaFree)
 template <class T>
-static cudaError_t upload_into(hk_context* ctx, hk_context::DevBuf& b, const T** dst, const T* src, size_t count) {
+static cudaError_t upload_into(hk_shared_scene* sc, hk_shared_scene::DevBuf& b, const T** dst, const T* src, size_t count) {
     const size_t bytes = count * sizeof(T), need = bytes + 64;   // +64: 16-byte vector loads at the tail stay in bounds
     cudaError_t e = cudaSuccess;
     if (b.cap < need) {
-        if (b.p) cudaFree(b.p);
+        if (b.p) { scene_before_free(sc); cudaFree(b.p); }
         b.p = nullptr; b.cap = 0;
         const size_t cap = need + need / 2;
         e = cudaMalloc(&b.p, cap);
         if (e != cudaSuccess) return e;
         b.cap = cap;
     }
-    if (bytes) e = cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(static_cast<char*>(b.p) + bytes, 0, 64, ctx->stream);
+    if (bytes) e = cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, sc->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(static_cast<char*>(b.p) + bytes, 0, 64, sc->stream);
     *dst = reinterpret_cast<const T*>(b.p);
     return e;
 }
 
 // The 4-wide tree over the instances (the half of upload_wide that every instance update repeats) from the flat TLAS in `nodes`
 // (host memory) and the instances' boxes (6 floats each, or null when the navigators carry them by construction); the meshes' trees
-// and ctx->wide_mesh_of are those of the last upload_wide.
-static int upload_wide_tlas(hk_context* ctx, const hk_node* nodes, uint32_t node_count, uint32_t instance_count, const float* instance_box,
+// and sc->wide_mesh_of are those of the last upload_wide.
+static int upload_wide_tlas(hk_shared_scene* sc, const hk_node* nodes, uint32_t node_count, uint32_t instance_count, const float* instance_box,
                             DeviceScene& d) {
     d.wide_ready = 0u; d.wide_tlas_root = WIDE_EMPTY;
     hkw::WideTree tlas = hkw::build_wide(nodes, node_count, instance_count, instance_box);
-    bool ok = tlas.ok && ctx->wide_mesh_of.size() == instance_count;
+    bool ok = tlas.ok && sc->wide_mesh_of.size() == instance_count;
     uint32_t blas_need = 0;
     std::vector<uint2> entry(instance_count);
-    for (uint32_t i = 0; i < instance_count && ctx->wide_mesh_of.size() == instance_count; ++i) {
-        const hk_context::WideMesh& m = ctx->wide_meshes[ctx->wide_mesh_of[i]];
+    for (uint32_t i = 0; i < instance_count && sc->wide_mesh_of.size() == instance_count; ++i) {
+        const hk_shared_scene::WideMesh& m = sc->wide_meshes[sc->wide_mesh_of[i]];
         ok = ok && m.ok;
         entry[i] = make_uint2(m.base, m.root);
         blas_need = std::max(blas_need, m.need);
     }
     if (!tlas.ok) { tlas.nodes.clear(); tlas.rank.assign(instance_count, 0u); }
-    ctx->wide_tlas_node_count = (uint32_t)tlas.nodes.size();
-    HK_CUDA(upload_into(ctx, ctx->ibuf[9], &d.wide_tlas, tlas.nodes.data(), tlas.nodes.size()));
-    HK_CUDA(upload_into(ctx, ctx->ibuf[11], &d.wide_instance, entry.data(), entry.size()));
-    HK_CUDA(upload_into(ctx, ctx->ibuf[12], &d.wide_instance_rank, tlas.rank.data(), tlas.rank.size()));
-    HK_CUDA(cudaStreamSynchronize(ctx->stream));
+    sc->wide_tlas_node_count = (uint32_t)tlas.nodes.size();
+    HK_SCUDA(upload_into(sc, sc->ibuf[9], &d.wide_tlas, tlas.nodes.data(), tlas.nodes.size()));
+    HK_SCUDA(upload_into(sc, sc->ibuf[11], &d.wide_instance, entry.data(), entry.size()));
+    HK_SCUDA(upload_into(sc, sc->ibuf[12], &d.wide_instance_rank, tlas.rank.data(), tlas.rank.size()));
+    HK_SCUDA(cudaStreamSynchronize(sc->stream));
     // pending TLAS siblings + the BLAS marker + pending BLAS siblings, and the three pushes a node step makes before it pops
-    ctx->wide_stack_need = tlas.stack_need + 1u + blas_need + 3u;
-    if (ok && ctx->wide_stack_need <= (uint32_t)HK_WIDE_STACK) {
+    sc->wide_stack_need = tlas.stack_need + 1u + blas_need + 3u;
+    if (ok && sc->wide_stack_need <= (uint32_t)HK_WIDE_STACK) {
         d.wide_tlas_root = tlas.root;
         d.wide_ready = 1u;
     }
@@ -506,9 +614,9 @@ static int upload_wide_tlas(hk_context* ctx, const hk_node* nodes, uint32_t node
 // (rebuilt only when the set of meshes in use changes), one over the instances (every call), the per-instance entry points and the
 // array-order ranks that settle ties.  d.wide_ready stays 0 — and every launch keeps the reference's walk — when a flat array is not
 // in bvh 0.7.1's layout or the trees could ask for more stack than the walk has.
-static int upload_wide(hk_context* ctx, const hk_scene_desc* s, DeviceScene& d) {
+static int upload_wide(hk_shared_scene* sc, const hk_scene_desc* s, DeviceScene& d) {
     d.wide_ready = 0u; d.wide_tlas_root = WIDE_EMPTY;
-    ctx->wide_stack_need = 0;
+    sc->wide_stack_need = 0;
     std::vector<std::array<uint32_t, 3>> keys;
     std::vector<uint32_t> mesh_of(s->instance_count);
     for (uint32_t i = 0; i < s->instance_count; ++i) {
@@ -519,16 +627,16 @@ static int upload_wide(hk_context* ctx, const hk_scene_desc* s, DeviceScene& d) 
         if (k == keys.size()) keys.push_back(key);
         mesh_of[i] = (uint32_t)k;
     }
-    if (keys != ctx->wide_mesh_keys || ctx->ibuf[10].p == nullptr) {
+    if (keys != sc->wide_mesh_keys || sc->ibuf[10].p == nullptr) {
         std::vector<hk_wide_node> all;
-        std::vector<hk_context::WideMesh> meshes(keys.size());
-        std::vector<uint32_t> prim_rank(ctx->scene_primitive_count, 0u);
+        std::vector<hk_shared_scene::WideMesh> meshes(keys.size());
+        std::vector<uint32_t> prim_rank(sc->scene_primitive_count, 0u);
         for (size_t k = 0; k < keys.size(); ++k) {
-            const hk_node* flat = ctx->host_asset_nodes.data() + keys[k][0];
+            const hk_node* flat = sc->host_asset_nodes.data() + keys[k][0];
             uint32_t shapes = 0;
             for (uint32_t r = 0; r < keys[k][1]; ++r)
                 if (flat[r].entry_index >= 0x80000000u) shapes = std::max(shapes, flat[r].entry_index - 0x80000000u + 1u);
-            hkw::WideTree t = hkw::build_wide(flat, keys[k][1], shapes, ctx->host_primitive_box.data() + 6 * (size_t)keys[k][2]);
+            hkw::WideTree t = hkw::build_wide(flat, keys[k][1], shapes, sc->host_primitive_box.data() + 6 * (size_t)keys[k][2]);
             meshes[k].ok = t.ok;
             if (!t.ok) continue;
             if (t.root == WIDE_EMPTY) {      // a mesh without records: WIDE_EMPTY as its entry point would end the whole walk, not
@@ -540,93 +648,93 @@ static int upload_wide(hk_context* ctx, const hk_scene_desc* s, DeviceScene& d) 
             for (uint32_t sh = 0; sh < shapes; ++sh)
                 if (t.rank[sh] != 0xFFFFFFFFu && (uint64_t)keys[k][2] + sh < prim_rank.size()) prim_rank[keys[k][2] + sh] = t.rank[sh];
         }
-        HK_CUDA(upload_into(ctx, ctx->ibuf[10], &d.wide_blas, all.data(), all.size()));
-        HK_CUDA(upload_into(ctx, ctx->ibuf[13], &d.wide_primitive_rank, prim_rank.data(), prim_rank.size()));
-        HK_CUDA(cudaStreamSynchronize(ctx->stream));      // the staging vectors die at the end of this block
-        ctx->wide_mesh_keys = keys; ctx->wide_meshes = meshes; ctx->wide_blas_node_count = (uint32_t)all.size();
+        HK_SCUDA(upload_into(sc, sc->ibuf[10], &d.wide_blas, all.data(), all.size()));
+        HK_SCUDA(upload_into(sc, sc->ibuf[13], &d.wide_primitive_rank, prim_rank.data(), prim_rank.size()));
+        HK_SCUDA(cudaStreamSynchronize(sc->stream));      // the staging vectors die at the end of this block
+        sc->wide_mesh_keys = keys; sc->wide_meshes = meshes; sc->wide_blas_node_count = (uint32_t)all.size();
     } else {
-        d.wide_blas = reinterpret_cast<const hk_wide_node*>(ctx->ibuf[10].p);
-        d.wide_primitive_rank = reinterpret_cast<const uint32_t*>(ctx->ibuf[13].p);
+        d.wide_blas = reinterpret_cast<const hk_wide_node*>(sc->ibuf[10].p);
+        d.wide_primitive_rank = reinterpret_cast<const uint32_t*>(sc->ibuf[13].p);
     }
-    ctx->wide_mesh_of = mesh_of;
+    sc->wide_mesh_of = mesh_of;
     std::vector<float> instance_box(6 * (size_t)s->instance_count);
     for (uint32_t i = 0; i < s->instance_count; ++i)
         for (int c = 0; c < 3; ++c) { instance_box[6 * (size_t)i + c] = s->instances[i].min[c]; instance_box[6 * (size_t)i + 3 + c] = s->instances[i].max[c]; }
-    return upload_wide_tlas(ctx, s->instance_nodes, s->instance_node_count, s->instance_count, instance_box.data(), d);
+    return upload_wide_tlas(sc, s->instance_nodes, s->instance_node_count, s->instance_count, instance_box.data(), d);
 }
 
 // Validation + upload of the per-frame half of the scene (instances, TLAS, emissives, emissive BVH, alias tables,
 // previous model matrices) into `d`.  Frees the previous copies.
-static int upload_instances(hk_context* ctx, const hk_scene_desc* s, DeviceScene& d) {
+static int upload_instances(hk_shared_scene* sc, const hk_scene_desc* s, DeviceScene& d) {
     // materials travel with the per-frame half when given (material.rs:139-203 rewrites them whenever a material changes)
     const bool new_materials = s->materials != nullptr && s->material_count > 0;
-    const uint32_t material_count = new_materials ? s->material_count : ctx->scene_material_count;
+    const uint32_t material_count = new_materials ? s->material_count : sc->scene_material_count;
     if ((s->instance_count && !s->instances) || (s->instance_node_count && !s->instance_nodes) ||
         (s->emissive_node_count && !s->emissive_nodes) || (s->emissive_count && !s->emissives) || (s->alias_count && !s->alias_table))
-        return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "scene buffer pointer is NULL with a non-zero count");
+        return set_error(sc, HK_ERR_INVALID_ARGUMENT, "scene buffer pointer is NULL with a non-zero count");
     // Validate every index the kernels follow, once, so that they can skip bounds checks (wgpu's robust buffer access would clamp
     // a bad index; here a malformed host buffer is refused instead of read out of bounds).
     for (uint32_t i = 0; i < s->instance_count; ++i) {
         const hk_instance& in = s->instances[i];
-        if (in.material >= material_count || (uint64_t)in.mesh.node_offset + in.mesh.node_count > ctx->scene_asset_node_count)
-            return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "instance references a material / node range out of bounds");
-        if (in.mesh.primitive > ctx->scene_primitive_count || in.mesh.vertex > ctx->scene_vertex_count)
-            return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "instance references a primitive / vertex range out of bounds");
+        if (in.material >= material_count || (uint64_t)in.mesh.node_offset + in.mesh.node_count > sc->scene_asset_node_count)
+            return set_error(sc, HK_ERR_INVALID_ARGUMENT, "instance references a material / node range out of bounds");
+        if (in.mesh.primitive > sc->scene_primitive_count || in.mesh.vertex > sc->scene_vertex_count)
+            return set_error(sc, HK_ERR_INVALID_ARGUMENT, "instance references a primitive / vertex range out of bounds");
         // every leaf of the instance's BLAS must name a primitive inside the primitive buffer, and every link a record of its range
         const std::array<uint32_t, 4> mesh_key = {in.mesh.vertex, in.mesh.primitive, in.mesh.node_offset, in.mesh.node_count};
-        if (!ctx->mesh_range_checked.count(mesh_key)) {
-            const std::vector<hk_node>& nodes = ctx->host_asset_nodes;
+        if (!sc->mesh_range_checked.count(mesh_key)) {
+            const std::vector<hk_node>& nodes = sc->host_asset_nodes;
             for (uint32_t k = 0; k < in.mesh.node_count; ++k) {
                 const hk_node& nd = nodes[in.mesh.node_offset + k];
                 if (nd.entry_index >= 0x80000000u) {
                     const uint64_t pid = (uint64_t)in.mesh.primitive + (nd.entry_index - 0x80000000u);
-                    if (pid >= ctx->scene_primitive_count)
-                        return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "BLAS leaf references a primitive out of bounds");
-                    const uint32_t* vi = &ctx->host_primitive_vertex_index[3 * pid];
+                    if (pid >= sc->scene_primitive_count)
+                        return set_error(sc, HK_ERR_INVALID_ARGUMENT, "BLAS leaf references a primitive out of bounds");
+                    const uint32_t* vi = &sc->host_primitive_vertex_index[3 * pid];
                     for (int c = 0; c < 3; ++c)
-                        if ((uint64_t)in.mesh.vertex + vi[c] >= ctx->scene_vertex_count)
-                            return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "primitive references a vertex out of bounds");
+                        if ((uint64_t)in.mesh.vertex + vi[c] >= sc->scene_vertex_count)
+                            return set_error(sc, HK_ERR_INVALID_ARGUMENT, "primitive references a vertex out of bounds");
                 } else if (nd.entry_index > in.mesh.node_count) {
-                    return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "BLAS entry link out of its mesh's node range");
+                    return set_error(sc, HK_ERR_INVALID_ARGUMENT, "BLAS entry link out of its mesh's node range");
                 }
             }
-            ctx->mesh_range_checked.insert(mesh_key);
+            sc->mesh_range_checked.insert(mesh_key);
         }
     }
-    if (new_materials && ctx->scene_texture_count != 0xFFFFFFFFu) {
+    if (new_materials && sc->scene_texture_count != 0xFFFFFFFFu) {
         for (uint32_t i = 0; i < s->material_count; ++i) {
             const hk_material& m = s->materials[i];
             const uint32_t ids[5] = {m.base_color_texture, m.emissive_texture, m.metallic_roughness_texture, m.normal_map_texture, m.occlusion_texture};
             for (uint32_t id : ids)
-                if (id != 0xFFFFFFFFu && id >= ctx->scene_texture_count)
-                    return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "material references a texture out of bounds");
+                if (id != 0xFFFFFFFFu && id >= sc->scene_texture_count)
+                    return set_error(sc, HK_ERR_INVALID_ARGUMENT, "material references a texture out of bounds");
         }
     }
     for (uint32_t i = 0; i < s->instance_node_count; ++i) {
         const hk_node& nd = s->instance_nodes[i];
         if (nd.entry_index >= 0x80000000u) {
             if (nd.entry_index - 0x80000000u >= s->instance_count)
-                return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "TLAS leaf references an instance out of bounds");
+                return set_error(sc, HK_ERR_INVALID_ARGUMENT, "TLAS leaf references an instance out of bounds");
         }
     }
     for (uint32_t i = 0; i < s->emissive_node_count; ++i) {
         const hk_node& nd = s->emissive_nodes[i];
         if (nd.entry_index >= 0x80000000u && nd.entry_index - 0x80000000u >= s->emissive_count)
-            return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "emissive BVH leaf references an emissive out of bounds");
+            return set_error(sc, HK_ERR_INVALID_ARGUMENT, "emissive BVH leaf references an emissive out of bounds");
     }
     for (uint32_t i = 0; i < s->emissive_count; ++i) {
         const hk_emissive& em = s->emissives[i];
         if (em.instance >= s->instance_count || (uint64_t)em.alias_table_offset + em.alias_table_count > s->alias_count || em.alias_table_count == 0)
-            return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "emissive references an instance / alias-table slice out of bounds");
+            return set_error(sc, HK_ERR_INVALID_ARGUMENT, "emissive references an instance / alias-table slice out of bounds");
         // alias entries index triangles of the emissive instance's mesh
         const hk_instance& ei = s->instances[em.instance];
         for (uint32_t k = 0; k < em.alias_table_count; ++k)
-            if ((uint64_t)ei.mesh.primitive + s->alias_table[em.alias_table_offset + k].index >= ctx->scene_primitive_count)
-                return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "alias-table entry references a primitive out of bounds");
+            if ((uint64_t)ei.mesh.primitive + s->alias_table[em.alias_table_offset + k].index >= sc->scene_primitive_count)
+                return set_error(sc, HK_ERR_INVALID_ARGUMENT, "alias-table entry references a primitive out of bounds");
     }
     // Does every leaf record sit right behind a navigator whose box is the shape's own AABB?  (true for bvh 0.7.1's
     // flatten_custom, which is what the reference uploads; then the kernels skip the re-derived leaf box test.)
-    bool boxes_match = ctx->mesh_boxes_match;
+    bool boxes_match = sc->mesh_boxes_match;
     auto same3 = [](const float* a, const float* b) { return a[0] == b[0] && a[1] == b[1] && a[2] == b[2]; };
     for (uint32_t i = 1; i < s->instance_node_count && boxes_match; ++i) {
         const hk_node& leaf = s->instance_nodes[i];
@@ -636,17 +744,17 @@ static int upload_instances(hk_context* ctx, const hk_scene_desc* s, DeviceScene
         boxes_match = nav.entry_index == i && id < s->instance_count && same3(nav.min, s->instances[id].min) &&
                       same3(nav.max, s->instances[id].max);
     }
-    HK_CUDA(cudaStreamSynchronize(ctx->stream));   // frames in flight still read the buffers that are overwritten below
+    HK_SCUDA(cudaStreamSynchronize(sc->stream));   // frames in flight still read the buffers that are overwritten below
     d.leaf_boxes_match = boxes_match ? 1u : 0u;
     if (new_materials) {
-        HK_CUDA(upload_into(ctx, ctx->ibuf[7], &d.materials, s->materials, s->material_count));
-        ctx->scene_material_count = s->material_count;
+        HK_SCUDA(upload_into(sc, sc->ibuf[7], &d.materials, s->materials, s->material_count));
+        sc->scene_material_count = s->material_count;
     }
-    HK_CUDA(upload_into(ctx, ctx->ibuf[0], &d.alias_table, s->alias_table, s->alias_count));
-    HK_CUDA(upload_into(ctx, ctx->ibuf[1], &d.instances, s->instances, s->instance_count));
-    HK_CUDA(upload_into(ctx, ctx->ibuf[2], &d.instance_nodes, s->instance_nodes, s->instance_node_count));
-    HK_CUDA(upload_into(ctx, ctx->ibuf[3], &d.emissive_nodes, s->emissive_nodes, s->emissive_node_count));
-    HK_CUDA(upload_into(ctx, ctx->ibuf[4], &d.emissives, s->emissives, s->emissive_count));
+    HK_SCUDA(upload_into(sc, sc->ibuf[0], &d.alias_table, s->alias_table, s->alias_count));
+    HK_SCUDA(upload_into(sc, sc->ibuf[1], &d.instances, s->instances, s->instance_count));
+    HK_SCUDA(upload_into(sc, sc->ibuf[2], &d.instance_nodes, s->instance_nodes, s->instance_node_count));
+    HK_SCUDA(upload_into(sc, sc->ibuf[3], &d.emissive_nodes, s->emissive_nodes, s->emissive_node_count));
+    HK_SCUDA(upload_into(sc, sc->ibuf[4], &d.emissives, s->emissives, s->emissive_count));
     {   // compact traversal records + what the pooled kernels stage into shared memory (hk_pool.cuh)
         std::vector<hk_instance_trav> trav(s->instance_count);
         for (uint32_t i = 0; i < s->instance_count; ++i) {
@@ -654,18 +762,18 @@ static int upload_instances(hk_context* ctx, const hk_scene_desc* s, DeviceScene
             trav[i].mesh[0] = s->instances[i].mesh.vertex; trav[i].mesh[1] = s->instances[i].mesh.primitive;
             trav[i].mesh[2] = s->instances[i].mesh.node_offset; trav[i].mesh[3] = s->instances[i].mesh.node_count;
         }
-        HK_CUDA(upload_into(ctx, ctx->ibuf[8], &d.instance_trav, trav.data(), trav.size()));
-        HK_CUDA(cudaStreamSynchronize(ctx->stream));      // `trav` dies at the end of this block
+        HK_SCUDA(upload_into(sc, sc->ibuf[8], &d.instance_trav, trav.data(), trav.size()));
+        HK_SCUDA(cudaStreamSynchronize(sc->stream));      // `trav` dies at the end of this block
         StagePlan plan{};
         const uint32_t budget = (uint32_t)HK_STAGE_F4;
         const uint64_t tlas = 2ull * s->instance_node_count, itrav = 5ull * s->instance_count;
         if (s->instance_node_count && tlas + itrav <= budget) {
             plan.tlas_f4 = 0; plan.tlas_count = s->instance_node_count;
             plan.itrav_f4 = (uint32_t)tlas; plan.itrav_count = s->instance_count;
-            const uint64_t used = tlas + itrav, blas = 2ull * ctx->scene_asset_node_count, prim = 3ull * ctx->scene_primitive_count;
-            if (ctx->scene_asset_node_count && used + blas + prim <= budget) {     // small scene: walked entirely out of shared memory
-                plan.blas_f4 = (uint32_t)used; plan.blas_count = ctx->scene_asset_node_count;
-                plan.prim_f4 = (uint32_t)(used + blas); plan.prim_count = ctx->scene_primitive_count;
+            const uint64_t used = tlas + itrav, blas = 2ull * sc->scene_asset_node_count, prim = 3ull * sc->scene_primitive_count;
+            if (sc->scene_asset_node_count && used + blas + prim <= budget) {     // small scene: walked entirely out of shared memory
+                plan.blas_f4 = (uint32_t)used; plan.blas_count = sc->scene_asset_node_count;
+                plan.prim_f4 = (uint32_t)(used + blas); plan.prim_count = sc->scene_primitive_count;
             }
         }
         d.stage = plan;
@@ -683,23 +791,20 @@ static int upload_instances(hk_context* ctx, const hk_scene_desc* s, DeviceScene
             any = any || moved[i];
         }
         if (any) {
-            HK_CUDA(upload_into(ctx, ctx->ibuf[5], &d.previous_models, reinterpret_cast<const float4*>(s->previous_instance_models), 4 * (size_t)s->instance_count));
-            HK_CUDA(upload_into(ctx, ctx->ibuf[6], &d.instance_moved, moved.data(), s->instance_count));
+            HK_SCUDA(upload_into(sc, sc->ibuf[5], &d.previous_models, reinterpret_cast<const float4*>(s->previous_instance_models), 4 * (size_t)s->instance_count));
+            HK_SCUDA(upload_into(sc, sc->ibuf[6], &d.instance_moved, moved.data(), s->instance_count));
         }
     }
-    HK_CUDA(cudaStreamSynchronize(ctx->stream));      // caller's arrays (and `moved`) may be freed after return
-    ctx->scene_instance_count = s->instance_count;
-    ctx->scene_emissive_count = s->emissive_count;
-    return upload_wide(ctx, s, d);
+    HK_SCUDA(cudaStreamSynchronize(sc->stream));      // caller's arrays (and `moved`) may be freed after return
+    sc->scene_instance_count = s->instance_count;
+    sc->scene_emissive_count = s->emissive_count;
+    return upload_wide(sc, s, d);
 }
 
-extern "C" {
-
-int hk_scene_upload(hk_context* ctx, const hk_scene_desc* s) {
-    if (!ctx || !s) return HK_ERR_INVALID_ARGUMENT;
+static int scene_upload(hk_shared_scene* sc, const hk_scene_desc* s) {
     if ((s->vertex_count && !s->vertices) || (s->primitive_count && !s->primitives) ||
         (s->material_count && !s->materials) || (s->asset_node_count && !s->asset_nodes) || (s->texture_count && !s->textures))
-        return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "scene buffer pointer is NULL with a non-zero count");
+        return set_error(sc, HK_ERR_INVALID_ARGUMENT, "scene buffer pointer is NULL with a non-zero count");
     bool boxes_match = true;
     auto same3 = [](const float* a, const float* b) { return a[0] == b[0] && a[1] == b[1] && a[2] == b[2]; };
     std::unordered_set<uint32_t> checked;   // mesh node ranges repeat across instances: check each once
@@ -722,36 +827,36 @@ int hk_scene_upload(hk_context* ctx, const hk_scene_desc* s) {
             boxes_match = same3(nav.min, mn) && same3(nav.max, mx);
         }
     }
-    HK_CUDA(cudaSetDevice(ctx->device));
-    HK_CUDA(cudaStreamSynchronize(ctx->stream));
-    free_list(ctx->scene_allocations);
-    ctx->scene_ready = false;
-    ctx->mesh_boxes_match = boxes_match;
-    ctx->scene_material_count = 0;
-    ctx->scene_asset_node_count = s->asset_node_count;
-    ctx->scene_primitive_count = s->primitive_count;
-    ctx->scene_vertex_count = s->vertex_count;
-    ctx->scene_texture_count = s->texture_count;
-    ctx->host_asset_nodes.assign(s->asset_nodes, s->asset_nodes + s->asset_node_count);
-    ctx->mesh_range_checked.clear();
-    ctx->wide_mesh_keys.clear(); ctx->wide_meshes.clear();     // new asset nodes: the meshes' 4-wide trees are rebuilt
-    ctx->host_primitive_vertex_index.resize(3 * (size_t)s->primitive_count);
+    HK_SCUDA(cudaSetDevice(sc->device));
+    HK_SCUDA(cudaStreamSynchronize(sc->stream));     // (after scene_begin_write: also every attached camera's last read)
+    free_list(sc->scene_allocations);
+    sc->ready = false;
+    sc->mesh_boxes_match = boxes_match;
+    sc->scene_material_count = 0;
+    sc->scene_asset_node_count = s->asset_node_count;
+    sc->scene_primitive_count = s->primitive_count;
+    sc->scene_vertex_count = s->vertex_count;
+    sc->scene_texture_count = s->texture_count;
+    sc->host_asset_nodes.assign(s->asset_nodes, s->asset_nodes + s->asset_node_count);
+    sc->mesh_range_checked.clear();
+    sc->wide_mesh_keys.clear(); sc->wide_meshes.clear();     // new asset nodes: the meshes' 4-wide trees are rebuilt
+    sc->host_primitive_vertex_index.resize(3 * (size_t)s->primitive_count);
     for (uint32_t i = 0; i < s->primitive_count; ++i)
-        for (int c = 0; c < 3; ++c) ctx->host_primitive_vertex_index[3 * (size_t)i + c] = s->primitives[i].vertices[c].index;
-    ctx->host_primitive_box.resize(6 * (size_t)s->primitive_count);
+        for (int c = 0; c < 3; ++c) sc->host_primitive_vertex_index[3 * (size_t)i + c] = s->primitives[i].vertices[c].index;
+    sc->host_primitive_box.resize(6 * (size_t)s->primitive_count);
     for (uint32_t i = 0; i < s->primitive_count; ++i) {
         const hk_primitive& p = s->primitives[i];
         for (int c = 0; c < 3; ++c) {
-            ctx->host_primitive_box[6 * (size_t)i + c] = fminf(p.vertices[0].position[c], fminf(p.vertices[1].position[c], p.vertices[2].position[c]));
-            ctx->host_primitive_box[6 * (size_t)i + 3 + c] = fmaxf(p.vertices[0].position[c], fmaxf(p.vertices[1].position[c], p.vertices[2].position[c]));
+            sc->host_primitive_box[6 * (size_t)i + c] = fminf(p.vertices[0].position[c], fminf(p.vertices[1].position[c], p.vertices[2].position[c]));
+            sc->host_primitive_box[6 * (size_t)i + 3 + c] = fmaxf(p.vertices[0].position[c], fmaxf(p.vertices[1].position[c], p.vertices[2].position[c]));
         }
     }
     // primitives index vertices relative to their mesh's vertex base: the largest index of each mesh is checked per instance
     // below through mesh.vertex + index < vertex_count for the primitives of its leaves
     DeviceScene d{};
-    HK_CUDA(upload(ctx, &d.vertices, s->vertices, s->vertex_count));
-    HK_CUDA(upload(ctx, &d.primitives, s->primitives, s->primitive_count));
-    HK_CUDA(upload(ctx, &d.asset_nodes, s->asset_nodes, s->asset_node_count));
+    HK_SCUDA(upload(sc, &d.vertices, s->vertices, s->vertex_count));
+    HK_SCUDA(upload(sc, &d.primitives, s->primitives, s->primitive_count));
+    HK_SCUDA(upload(sc, &d.asset_nodes, s->asset_nodes, s->asset_node_count));
     d.materials = nullptr;           // uploaded with the per-frame half below
     d.texture_count = s->texture_count;
     d.textures = nullptr;
@@ -767,12 +872,12 @@ int hk_scene_upload(hk_context* ctx, const hk_scene_desc* s) {
         size_t total = 0;
         for (uint32_t t = 0; t < s->texture_count; ++t) {
             const hk_texture_desc& td = s->textures[t];
-            if (!td.rgba8 || !td.width || !td.height) return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "bad texture");
+            if (!td.rgba8 || !td.width || !td.height) return set_error(sc, HK_ERR_INVALID_ARGUMENT, "bad texture");
             info[t] = make_uint4((uint32_t)total, td.width, td.height,
                                  (td.address_mode_u & 3u) | ((td.address_mode_v & 3u) << 2) | (td.filter_linear ? 16u : 0u));
             total += (size_t)td.width * td.height;
         }
-        if (total > 0xFFFFFFFFull) return set_error(ctx, HK_ERR_UNSUPPORTED, "texture atlas too large");
+        if (total > 0xFFFFFFFFull) return set_error(sc, HK_ERR_UNSUPPORTED, "texture atlas too large");
         std::vector<float4> texels(total);
         for (uint32_t t = 0; t < s->texture_count; ++t) {
             const hk_texture_desc& td = s->textures[t];
@@ -782,38 +887,39 @@ int hk_scene_upload(hk_context* ctx, const hk_scene_desc* s) {
             for (size_t i = 0; i < n; ++i)
                 dst[i] = make_float4(lut[td.rgba8[4 * i]], lut[td.rgba8[4 * i + 1]], lut[td.rgba8[4 * i + 2]], lin_lut[td.rgba8[4 * i + 3]]);
         }
-        HK_CUDA(upload(ctx, &d.texture_texels, texels.data(), (uint32_t)total));
-        HK_CUDA(upload(ctx, &d.texture_info, info.data(), s->texture_count));
-        HK_CUDA(cudaStreamSynchronize(ctx->stream));  // host staging vectors die at scope exit
+        HK_SCUDA(upload(sc, &d.texture_texels, texels.data(), (uint32_t)total));
+        HK_SCUDA(upload(sc, &d.texture_info, info.data(), s->texture_count));
+        HK_SCUDA(cudaStreamSynchronize(sc->stream));  // host staging vectors die at scope exit
     }
-    int rc = upload_instances(ctx, s, d);
+    int rc = upload_instances(sc, s, d);
     if (rc != HK_OK) return rc;
-    ctx->scene = d;
-    ctx->scene_ready = true;
+    sc->scene = d;
+    sc->ready = true;
     return HK_OK;
 }
 
-int hk_scene_update_instances(hk_context* ctx, const hk_scene_desc* s) {
-    if (!ctx || !s) return HK_ERR_INVALID_ARGUMENT;
-    if (!ctx->scene_ready) return set_error(ctx, HK_ERR_NOT_READY, "hk_scene_update_instances needs a scene from hk_scene_upload");
-    HK_CUDA(cudaSetDevice(ctx->device));
-    DeviceScene d = ctx->scene;
-    int rc = upload_instances(ctx, s, d);
+static int scene_update_instances(hk_shared_scene* sc, const hk_scene_desc* s) {
+    if (!sc->ready) return set_error(sc, HK_ERR_NOT_READY, "hk_scene_update_instances needs a scene from hk_scene_upload");
+    HK_SCUDA(cudaSetDevice(sc->device));
+    DeviceScene d = sc->scene;
+    int rc = upload_instances(sc, s, d);
     if (rc != HK_OK) {   // validation fails before anything is freed; a CUDA failure may leave freed buffers behind
-        if (rc != HK_ERR_INVALID_ARGUMENT) ctx->scene_ready = false;
+        if (rc != HK_ERR_INVALID_ARGUMENT) sc->ready = false;
         return rc;
     }
-    ctx->scene = d;
+    sc->scene = d;
     return HK_OK;
 }
 
+extern "C" {      // (defined with the scheduling below)
 static bool wide_primary(const hk_context* ctx);
 static bool wide_light(const hk_context* ctx);
+}
 // grow-only device scratch
-static cudaError_t ensure_buf(hk_context::DevBuf& b, size_t bytes) {
+static cudaError_t ensure_buf(hk_shared_scene* sc, hk_shared_scene::DevBuf& b, size_t bytes) {
     const size_t need = bytes + 64;
     if (b.cap >= need) return cudaSuccess;
-    if (b.p) cudaFree(b.p);
+    if (b.p) { scene_before_free(sc); cudaFree(b.p); }
     b.p = nullptr; b.cap = 0;
     const size_t cap = need + need / 2;
     cudaError_t e = cudaMalloc(&b.p, cap);
@@ -822,31 +928,31 @@ static cudaError_t ensure_buf(hk_context::DevBuf& b, size_t bytes) {
 }
 
 // SURVEY 8(f) rank 2 — the per-frame half of the scene rebuilt on the device (kernels_scene.cu) from the model matrices alone.
-int hk_scene_update_transforms(hk_context* ctx, const float* models, const float* previous_models, const float* mesh_aabbs, uint32_t instance_count) {
-    if (!ctx || (instance_count && (!models || !mesh_aabbs))) return HK_ERR_INVALID_ARGUMENT;
-    if (!ctx->scene_ready) return set_error(ctx, HK_ERR_NOT_READY, "hk_scene_update_transforms needs a scene from hk_scene_upload");
-    if (instance_count != ctx->scene_instance_count)
-        return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "hk_scene_update_transforms moves the instances of the last upload: their number must be unchanged "
+static int scene_update_transforms(hk_shared_scene* sc, const float* models, const float* previous_models, const float* mesh_aabbs,
+                                   uint32_t instance_count, uint32_t* launches) {
+    if (!sc->ready) return set_error(sc, HK_ERR_NOT_READY, "hk_scene_update_transforms needs a scene from hk_scene_upload");
+    if (instance_count != sc->scene_instance_count)
+        return set_error(sc, HK_ERR_INVALID_ARGUMENT, "hk_scene_update_transforms moves the instances of the last upload: their number must be unchanged "
                                                        "(a changed set goes through hk_scene_update_instances)");
-    const uint32_t n = instance_count, ne = ctx->scene_emissive_count;
+    const uint32_t n = instance_count, ne = sc->scene_emissive_count;
     if (n == 0u) return HK_OK;
-    DeviceScene d = ctx->scene;
+    DeviceScene d = sc->scene;
     // the arrays being rebuilt in place must have bvh 0.7.1's sizes (3 m - 2 records over m >= 2 shapes, 1 over one)
     const uint32_t tlas_records = n == 1u ? 1u : 3u * n - 2u, em_records = ne == 0u ? 0u : (ne == 1u ? 1u : 3u * ne - 2u);
     if (d.instance_node_count != tlas_records || d.emissive_node_count != em_records)
-        return set_error(ctx, HK_ERR_UNSUPPORTED, "the uploaded TLAS / emissive BVH is not in bvh 0.7.1's flatten_custom layout: use hk_scene_update_instances");
-    HK_CUDA(cudaSetDevice(ctx->device));
+        return set_error(sc, HK_ERR_UNSUPPORTED, "the uploaded TLAS / emissive BVH is not in bvh 0.7.1's flatten_custom layout: use hk_scene_update_instances");
+    HK_SCUDA(cudaSetDevice(sc->device));
     const size_t mbytes = 64u * (size_t)n, abytes = 24u * (size_t)n;
     const size_t stage_bytes = mbytes * (previous_models ? 2u : 1u) + abytes;
     // pinned staging: the caller's arrays are free on return and the host does not wait for the frames in flight
-    hk_context::PinBuf& pin = ctx->pin[ctx->pin_slot];
-    ctx->pin_slot ^= 1;
-    if (!pin.ev) HK_CUDA(cudaEventCreateWithFlags(&pin.ev, cudaEventDisableTiming));
-    if (pin.used) HK_CUDA(cudaEventSynchronize(pin.ev));          // the copy made from this slot two calls ago
+    hk_shared_scene::PinBuf& pin = sc->pin[sc->pin_slot];
+    sc->pin_slot ^= 1;
+    if (!pin.ev) HK_SCUDA(cudaEventCreateWithFlags(&pin.ev, cudaEventDisableTiming));
+    if (pin.used) HK_SCUDA(cudaEventSynchronize(pin.ev));          // the copy made from this slot two calls ago
     if (pin.cap < stage_bytes) {
         if (pin.p) cudaFreeHost(pin.p);
         pin.p = nullptr; pin.cap = 0;
-        HK_CUDA(cudaMallocHost(&pin.p, stage_bytes + stage_bytes / 2));
+        HK_SCUDA(cudaMallocHost(&pin.p, stage_bytes + stage_bytes / 2));
         pin.cap = stage_bytes + stage_bytes / 2;
     }
     // staging layout: models | previous models (optional) | mesh AABBs — the two matrix arrays are read as float4 and must stay
@@ -858,79 +964,207 @@ int hk_scene_update_transforms(hk_context* ctx, const float* models, const float
     if (previous_models) memcpy(hp + mbytes, previous_models, mbytes);
     memcpy(hp + aoff, mesh_aabbs, abytes);
     const uint32_t nmax = n > ne ? n : ne;
-    HK_CUDA(ensure_buf(ctx->ibuf[14], stage_bytes));
-    HK_CUDA(ensure_buf(ctx->ibuf[5], mbytes));
-    HK_CUDA(ensure_buf(ctx->ibuf[6], 4u * (size_t)n));
-    HK_CUDA(ensure_buf(ctx->ibuf[17], 16u * (size_t)nmax));
-    HK_CUDA(ensure_buf(ctx->ibuf[18], 16u * (size_t)nmax));
-    HK_CUDA(ensure_buf(ctx->ibuf[19], hk_scene_bvh_scratch_bytes(nmax)));
-    uint8_t* dp = static_cast<uint8_t*>(ctx->ibuf[14].p);
-    HK_CUDA(cudaMemcpyAsync(dp, hp, stage_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    HK_CUDA(cudaEventRecord(pin.ev, ctx->stream));
+    HK_SCUDA(ensure_buf(sc, sc->ibuf[14], stage_bytes));
+    HK_SCUDA(ensure_buf(sc, sc->ibuf[5], mbytes));
+    HK_SCUDA(ensure_buf(sc, sc->ibuf[6], 4u * (size_t)n));
+    HK_SCUDA(ensure_buf(sc, sc->ibuf[17], 16u * (size_t)nmax));
+    HK_SCUDA(ensure_buf(sc, sc->ibuf[18], 16u * (size_t)nmax));
+    HK_SCUDA(ensure_buf(sc, sc->ibuf[19], hk_scene_bvh_scratch_bytes(nmax)));
+    uint8_t* dp = static_cast<uint8_t*>(sc->ibuf[14].p);
+    HK_SCUDA(cudaMemcpyAsync(dp, hp, stage_bytes, cudaMemcpyHostToDevice, sc->stream));
+    HK_SCUDA(cudaEventRecord(pin.ev, sc->stream));
     pin.used = true;
-    hk_instance* instances = static_cast<hk_instance*>(ctx->ibuf[1].p);
-    hk_emissive* emissives = static_cast<hk_emissive*>(ctx->ibuf[4].p);
-    float4* box_lo = static_cast<float4*>(ctx->ibuf[17].p);
-    float4* box_hi = static_cast<float4*>(ctx->ibuf[18].p);
+    hk_instance* instances = static_cast<hk_instance*>(sc->ibuf[1].p);
+    hk_emissive* emissives = static_cast<hk_emissive*>(sc->ibuf[4].p);
+    float4* box_lo = static_cast<float4*>(sc->ibuf[17].p);
+    float4* box_hi = static_cast<float4*>(sc->ibuf[18].p);
     hk_launch_scene_instances(n, reinterpret_cast<const float4*>(dp), previous_models ? reinterpret_cast<const float4*>(dp + mbytes) : nullptr,
-                              reinterpret_cast<const float*>(dp + aoff), instances, static_cast<hk_instance_trav*>(ctx->ibuf[8].p),
-                              static_cast<float4*>(ctx->ibuf[5].p), static_cast<uint32_t*>(ctx->ibuf[6].p), box_lo, box_hi, ctx->stream);
-    hk_launch_build_flat_bvh(n, box_lo, box_hi, ctx->ibuf[19].p, static_cast<hk_node*>(ctx->ibuf[2].p),
-                             reinterpret_cast<uint8_t*>(instances) + offsetof(hk_instance, node_index), (uint32_t)sizeof(hk_instance), ctx->stream);
+                              reinterpret_cast<const float*>(dp + aoff), instances, static_cast<hk_instance_trav*>(sc->ibuf[8].p),
+                              static_cast<float4*>(sc->ibuf[5].p), static_cast<uint32_t*>(sc->ibuf[6].p), box_lo, box_hi, sc->stream);
+    hk_launch_build_flat_bvh(n, box_lo, box_hi, sc->ibuf[19].p, static_cast<hk_node*>(sc->ibuf[2].p),
+                             reinterpret_cast<uint8_t*>(instances) + offsetof(hk_instance, node_index), (uint32_t)sizeof(hk_instance), sc->stream);
     if (ne) {
-        hk_launch_scene_emissives(ne, emissives, instances, d.materials, d.primitives, d.vertices, box_lo, box_hi, ctx->stream);
-        hk_launch_build_flat_bvh(ne, box_lo, box_hi, ctx->ibuf[19].p, static_cast<hk_node*>(ctx->ibuf[3].p),
-                                 reinterpret_cast<uint8_t*>(emissives) + offsetof(hk_emissive, node_index), (uint32_t)sizeof(hk_emissive), ctx->stream);
+        hk_launch_scene_emissives(ne, emissives, instances, d.materials, d.primitives, d.vertices, box_lo, box_hi, sc->stream);
+        hk_launch_build_flat_bvh(ne, box_lo, box_hi, sc->ibuf[19].p, static_cast<hk_node*>(sc->ibuf[3].p),
+                                 reinterpret_cast<uint8_t*>(emissives) + offsetof(hk_emissive, node_index), (uint32_t)sizeof(hk_emissive), sc->stream);
     }
-    HK_CUDA(cudaGetLastError());
-    ctx->launches += ne ? 4u : 2u;
-    d.previous_models = static_cast<const float4*>(ctx->ibuf[5].p);
-    d.instance_moved = static_cast<const uint32_t*>(ctx->ibuf[6].p);
-    d.leaf_boxes_match = ctx->mesh_boxes_match ? 1u : 0u;       // every navigator carries its instance's own box by construction
+    HK_SCUDA(cudaGetLastError());
+    *launches = ne ? 4u : 2u;
+    d.previous_models = static_cast<const float4*>(sc->ibuf[5].p);
+    d.instance_moved = static_cast<const uint32_t*>(sc->ibuf[6].p);
+    d.leaf_boxes_match = sc->mesh_boxes_match ? 1u : 0u;       // every navigator carries its instance's own box by construction
     d.wide_ready = 0u; d.wide_tlas_root = WIDE_EMPTY;
-    if (wide_primary(ctx) || wide_light(ctx)) {
+    bool wide = false;          // the 4-wide TLAS is re-derived when any attached camera walks the wide trees
+    for (const hk_context* c : sc->attached) wide = wide || wide_primary(c) || wide_light(c);
+    if (wide) {
         // image-exact traversal mode in use: its 4-wide TLAS is derived on the host from the records just built (one small read-back;
         // scenes that walk the reference's arrays never reach this and never synchronise)
         std::vector<hk_node> nodes(tlas_records);
-        HK_CUDA(cudaMemcpyAsync(nodes.data(), ctx->ibuf[2].p, sizeof(hk_node) * (size_t)tlas_records, cudaMemcpyDeviceToHost, ctx->stream));
-        HK_CUDA(cudaStreamSynchronize(ctx->stream));
-        int rc = upload_wide_tlas(ctx, nodes.data(), tlas_records, n, nullptr, d);     // leaf navigators = instance boxes, as built
+        HK_SCUDA(cudaMemcpyAsync(nodes.data(), sc->ibuf[2].p, sizeof(hk_node) * (size_t)tlas_records, cudaMemcpyDeviceToHost, sc->stream));
+        HK_SCUDA(cudaStreamSynchronize(sc->stream));
+        int rc = upload_wide_tlas(sc, nodes.data(), tlas_records, n, nullptr, d);     // leaf navigators = instance boxes, as built
         if (rc != HK_OK) return rc;
     }
-    ctx->scene = d;
+    sc->scene = d;
     return HK_OK;
 }
 
 // Test / debugging aid: the per-frame scene buffers as they are on the device (what hk_scene_update_transforms built in place).
-static bool scene_buffer(const hk_context* ctx, int which, const void** src, size_t* have) {
-    const DeviceScene& d = ctx->scene;
+static bool scene_buffer(const hk_shared_scene* sc, int which, const void** src, size_t* have) {
+    const DeviceScene& d = sc->scene;
     switch (which) {
-        case HK_SCENE_INSTANCES: *src = d.instances; *have = sizeof(hk_instance) * (size_t)ctx->scene_instance_count; return true;
+        case HK_SCENE_INSTANCES: *src = d.instances; *have = sizeof(hk_instance) * (size_t)sc->scene_instance_count; return true;
         case HK_SCENE_INSTANCE_NODES: *src = d.instance_nodes; *have = sizeof(hk_node) * (size_t)d.instance_node_count; return true;
-        case HK_SCENE_EMISSIVES: *src = d.emissives; *have = sizeof(hk_emissive) * (size_t)ctx->scene_emissive_count; return true;
+        case HK_SCENE_EMISSIVES: *src = d.emissives; *have = sizeof(hk_emissive) * (size_t)sc->scene_emissive_count; return true;
         case HK_SCENE_EMISSIVE_NODES: *src = d.emissive_nodes; *have = sizeof(hk_node) * (size_t)d.emissive_node_count; return true;
-        case HK_SCENE_PREVIOUS_MODELS: *src = d.previous_models; *have = d.previous_models ? 64u * (size_t)ctx->scene_instance_count : 0u; return true;
-        case HK_SCENE_INSTANCE_MOVED: *src = d.instance_moved; *have = d.instance_moved ? 4u * (size_t)ctx->scene_instance_count : 0u; return true;
+        case HK_SCENE_PREVIOUS_MODELS: *src = d.previous_models; *have = d.previous_models ? 64u * (size_t)sc->scene_instance_count : 0u; return true;
+        case HK_SCENE_INSTANCE_MOVED: *src = d.instance_moved; *have = d.instance_moved ? 4u * (size_t)sc->scene_instance_count : 0u; return true;
         default: return false;
     }
 }
+
+// The scene that a context's hk_scene_upload / hk_scene_update_* write: its private one.  A context rendering a shared scene is
+// refused (the scene is updated through its handle); a context without a scene gets a private one on its own stream at upload.
+static int private_scene(hk_context* ctx, bool create, hk_shared_scene** out) {
+    *out = nullptr;
+    if (ctx->sc && ctx->sc->owner != ctx)
+        return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "the context renders a shared scene: upload and update it through its hk_shared_scene handle");
+    if (!ctx->sc && create) {
+        hk_shared_scene* sc = new hk_shared_scene();
+        sc->device = ctx->device;
+        sc->stream = ctx->stream;
+        sc->handle = false;
+        sc->owner = ctx;
+        attach_scene(ctx, sc);       // same stream: records nothing, cannot fail
+    }
+    *out = ctx->sc;
+    return HK_OK;
+}
+static int scene_result(hk_context* ctx, hk_shared_scene* sc, int rc) {   // a scene's error, reported on the context that asked
+    if (rc != HK_OK) ctx->error = sc->error;
+    return rc;
+}
+static int do_upload(hk_shared_scene* sc, const hk_scene_desc* s) {
+    scene_begin_write(sc);
+    const int rc = scene_upload(sc, s);
+    scene_end_write(sc);
+    return rc;
+}
+static int do_update_instances(hk_shared_scene* sc, const hk_scene_desc* s) {
+    if (!sc->ready) return set_error(sc, HK_ERR_NOT_READY, "hk_scene_update_instances needs a scene from hk_scene_upload");
+    scene_begin_write(sc);
+    const int rc = scene_update_instances(sc, s);
+    scene_end_write(sc);
+    return rc;
+}
+static int do_update_transforms(hk_shared_scene* sc, const float* models, const float* previous_models, const float* mesh_aabbs,
+                                uint32_t instance_count, uint32_t* launches) {
+    if (!sc->ready) return set_error(sc, HK_ERR_NOT_READY, "hk_scene_update_transforms needs a scene from hk_scene_upload");
+    scene_begin_write(sc);
+    const int rc = scene_update_transforms(sc, models, previous_models, mesh_aabbs, instance_count, launches);
+    scene_end_write(sc);
+    return rc;
+}
+
+extern "C" {
+
+int hk_scene_upload(hk_context* ctx, const hk_scene_desc* s) {
+    if (!ctx || !s) return HK_ERR_INVALID_ARGUMENT;
+    hk_shared_scene* sc = nullptr;
+    int rc = private_scene(ctx, true, &sc);
+    if (rc != HK_OK) return rc;
+    return scene_result(ctx, sc, do_upload(sc, s));
+}
+int hk_scene_update_instances(hk_context* ctx, const hk_scene_desc* s) {
+    if (!ctx || !s) return HK_ERR_INVALID_ARGUMENT;
+    hk_shared_scene* sc = nullptr;
+    int rc = private_scene(ctx, false, &sc);
+    if (rc != HK_OK) return rc;
+    if (!sc) return set_error(ctx, HK_ERR_NOT_READY, "hk_scene_update_instances needs a scene from hk_scene_upload");
+    return scene_result(ctx, sc, do_update_instances(sc, s));
+}
+int hk_scene_update_transforms(hk_context* ctx, const float* models, const float* previous_models, const float* mesh_aabbs, uint32_t instance_count) {
+    if (!ctx || (instance_count && (!models || !mesh_aabbs))) return HK_ERR_INVALID_ARGUMENT;
+    hk_shared_scene* sc = nullptr;
+    int rc = private_scene(ctx, false, &sc);
+    if (rc != HK_OK) return rc;
+    if (!sc) return set_error(ctx, HK_ERR_NOT_READY, "hk_scene_update_transforms needs a scene from hk_scene_upload");
+    uint32_t launches = 0;
+    rc = scene_result(ctx, sc, do_update_transforms(sc, models, previous_models, mesh_aabbs, instance_count, &launches));
+    ctx->launches += launches;
+    return rc;
+}
+
+int hk_shared_scene_create(hk_shared_scene** out, int cuda_device, void* cuda_stream) {
+    if (!out) return set_error(nullptr, HK_ERR_INVALID_ARGUMENT, "out == NULL");
+    *out = nullptr;
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    if (e != cudaSuccess || ndev == 0)
+        return set_error(nullptr, HK_ERR_CUDA, std::string("no CUDA device: ") + cudaGetErrorString(e) +
+                                                   " (this library has no CPU fallback)");
+    if (cuda_device < 0 || cuda_device >= ndev) return set_error(nullptr, HK_ERR_INVALID_ARGUMENT, "bad cuda_device");
+    e = cudaSetDevice(cuda_device);
+    if (e != cudaSuccess) return set_error(nullptr, HK_ERR_CUDA, cudaGetErrorString(e));
+    hk_shared_scene* sc = new hk_shared_scene();
+    sc->device = cuda_device;
+    if (cuda_stream) sc->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
+    else {
+        e = cudaStreamCreateWithFlags(&sc->stream, cudaStreamNonBlocking);
+        if (e != cudaSuccess) { delete sc; return set_error(nullptr, HK_ERR_CUDA, cudaGetErrorString(e)); }
+        sc->own_stream = true;
+    }
+    *out = sc;
+    return HK_OK;
+}
+void hk_shared_scene_destroy(hk_shared_scene* sc) {
+    if (!sc) return;
+    sc->handle = false;
+    if (sc->attached.empty()) scene_free(sc);
+}
+int hk_shared_scene_upload(hk_shared_scene* sc, const hk_scene_desc* s) {
+    if (!sc || !s) return HK_ERR_INVALID_ARGUMENT;
+    return do_upload(sc, s);
+}
+int hk_shared_scene_update_instances(hk_shared_scene* sc, const hk_scene_desc* s) {
+    if (!sc || !s) return HK_ERR_INVALID_ARGUMENT;
+    return do_update_instances(sc, s);
+}
+int hk_shared_scene_update_transforms(hk_shared_scene* sc, const float* models, const float* previous_models, const float* mesh_aabbs,
+                                      uint32_t instance_count) {
+    if (!sc || (instance_count && (!models || !mesh_aabbs))) return HK_ERR_INVALID_ARGUMENT;
+    uint32_t launches = 0;
+    return do_update_transforms(sc, models, previous_models, mesh_aabbs, instance_count, &launches);
+}
+const char* hk_shared_scene_last_error(hk_shared_scene* sc) { return sc ? sc->error.c_str() : g_create_error.c_str(); }
+
+int hk_context_attach_scene(hk_context* ctx, hk_shared_scene* sc) {
+    if (!ctx) return HK_ERR_INVALID_ARGUMENT;
+    if (sc && sc->device != ctx->device) return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "the scene lives on another device than the context");
+    if (sc && sc->owner) return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "a private scene cannot be attached to another context");
+    if (sc == ctx->sc) return HK_OK;
+    HK_CUDA(cudaSetDevice(ctx->device));
+    detach_scene(ctx);
+    return sc ? attach_scene(ctx, sc) : HK_OK;
+}
+
 int hk_scene_buffer_bytes(hk_context* ctx, int which, size_t* bytes) {
     if (!ctx || !bytes) return HK_ERR_INVALID_ARGUMENT;
-    if (!ctx->scene_ready) return set_error(ctx, HK_ERR_NOT_READY, "no scene");
+    if (!scene_ready(ctx)) return set_error(ctx, HK_ERR_NOT_READY, "no scene");
     const void* src = nullptr;
-    if (!scene_buffer(ctx, which, &src, bytes)) return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "unknown scene buffer");
+    if (!scene_buffer(ctx->sc, which, &src, bytes)) return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "unknown scene buffer");
     return HK_OK;
 }
 int hk_scene_readback(hk_context* ctx, int which, void* host, size_t bytes) {
     if (!ctx || (!host && bytes)) return HK_ERR_INVALID_ARGUMENT;
-    if (!ctx->scene_ready) return set_error(ctx, HK_ERR_NOT_READY, "no scene");
+    if (!scene_ready(ctx)) return set_error(ctx, HK_ERR_NOT_READY, "no scene");
     const void* src = nullptr;
     size_t have = 0;
-    if (!scene_buffer(ctx, which, &src, &have)) return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "unknown scene buffer");
+    if (!scene_buffer(ctx->sc, which, &src, &have)) return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "unknown scene buffer");
     if (bytes != have) return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "size mismatch");
     HK_CUDA(cudaSetDevice(ctx->device));
-    if (bytes) HK_CUDA(cudaMemcpyAsync(host, src, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    HK_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (bytes) HK_CUDA(cudaMemcpyAsync(host, src, bytes, cudaMemcpyDeviceToHost, ctx->sc->stream));   // behind the scene's updates
+    HK_CUDA(cudaStreamSynchronize(ctx->sc->stream));
     return HK_OK;
 }
 
@@ -948,7 +1182,7 @@ int hk_set_noise(hk_context* ctx, const uint8_t* rgba) {
 // ------------------------------------------------------------------------------------------------ scheduling
 static int make_params(hk_context* ctx, const hk_frame_inputs* in, KParams& P) {
     if (!ctx || !in) return HK_ERR_INVALID_ARGUMENT;
-    if (!ctx->scene_ready || !ctx->noise_ready) return set_error(ctx, HK_ERR_NOT_READY, "scene or noise not uploaded");
+    if (!scene_ready(ctx) || !ctx->noise_ready) return set_error(ctx, HK_ERR_NOT_READY, "scene or noise not uploaded");
     if (!ctx->planes_ready) return set_error(ctx, HK_ERR_NOT_READY, "per-pixel planes are not allocated (a resize failed)");
     const bool ratio1 = in->frame.upscale_ratio == 1.0f;
     if (!(in->frame.upscale_ratio >= 1.0f && in->frame.upscale_ratio <= 2.0f))
@@ -966,7 +1200,7 @@ static int make_params(hk_context* ctx, const hk_frame_inputs* in, KParams& P) {
         return set_error(ctx, HK_ERR_INVALID_ARGUMENT, "validate interval must be >= 1");
     if (cudaSetDevice(ctx->device) != cudaSuccess) return set_error(ctx, HK_ERR_CUDA, "cudaSetDevice");
     P.in = *in;
-    P.scene = ctx->scene;
+    P.scene = ctx->sc->scene;      // the attached scene as it is now (stream order: SceneUse)
     P.planes = ctx->planes;
     P.planes.pos_depth = ctx->planes.pos_depth_db[ctx->gbuffer_current];
     P.planes.velocity_uv = ctx->planes.velocity_uv_db[ctx->gbuffer_current];
@@ -1033,11 +1267,11 @@ static void rows(const hk_context* ctx, KParams& P, int ghost) {   // owned rect
 #define HK_WIDE_MIN_NODES 256
 #endif
 static bool wide_primary(const hk_context* ctx) {
-    if (!ctx->scene_ready || !ctx->scene.wide_ready) return false;
+    if (!scene_ready(ctx) || !ctx->sc->scene.wide_ready) return false;
     if (ctx->wide_traversal == 3) return true;
-    return ctx->wide_traversal == 1 && ctx->wide_blas_node_count + ctx->wide_tlas_node_count >= (uint32_t)HK_WIDE_MIN_NODES;
+    return ctx->wide_traversal == 1 && ctx->sc->wide_blas_node_count + ctx->sc->wide_tlas_node_count >= (uint32_t)HK_WIDE_MIN_NODES;
 }
-static bool wide_light(const hk_context* ctx) { return ctx->scene_ready && ctx->scene.wide_ready && ctx->wide_traversal == 3; }
+static bool wide_light(const hk_context* ctx) { return scene_ready(ctx) && ctx->sc->scene.wide_ready && ctx->wide_traversal == 3; }
 
 static int check_launch(hk_context* ctx) {
     cudaError_t e = cudaGetLastError();
@@ -1150,6 +1384,7 @@ static int run_post(hk_context* ctx, KParams& P, bool fuse) {  // PostProcessNod
 
 int hk_prepass_run(hk_context* ctx, const hk_frame_inputs* in) {
     KParams P; int rc = make_params(ctx, in, P); if (rc) return rc;
+    SceneUse use(ctx);
     ctx->launches = 0;
     return run_prepass(ctx, P);
 }
@@ -1181,6 +1416,7 @@ int hk_import_gbuffer(hk_context* ctx, const hk_gbuffer_desc* g) {
 }
 int hk_light_run(hk_context* ctx, const hk_frame_inputs* in) {
     KParams P; int rc = make_params(ctx, in, P); if (rc) return rc;
+    SceneUse use(ctx);
     ctx->launches = 0;
     // LightNode::run starts with full_screen_albedo (light.rs:645-653).  hk_render_frame has it fused into the G-buffer
     // kernel; the stand-alone node recomputes it from whatever G-buffer is current (e.g. one supplied with hk_upload_state).
@@ -1201,6 +1437,7 @@ int hk_post_process_run(hk_context* ctx, const hk_frame_inputs* in) {
 int hk_run_pass(hk_context* ctx, const hk_frame_inputs* in, int pass, int arg) {
     (void)arg;
     KParams P; int rc = make_params(ctx, in, P); if (rc) return rc;
+    SceneUse use(ctx);
     ctx->launches = 0;
     const hk_frame_uniform& f = P.in.frame;
     const int GS = ::GHOST_SPATIAL + ring_of(P), GT = GHOST_TEMPORAL + ctx->motion_margin;
@@ -1232,6 +1469,7 @@ int hk_run_pass(hk_context* ctx, const hk_frame_inputs* in, int pass, int arg) {
 }
 int hk_render_frame(hk_context* ctx, const hk_frame_inputs* in) {
     KParams P; int rc = make_params(ctx, in, P); if (rc) return rc;
+    SceneUse use(ctx);
     ctx->launches = 0;
     for (int i = 0; i < HK_K_COUNT; ++i) ctx->kran[i] = false;
     ctx->ring_hit = false;
@@ -1317,7 +1555,7 @@ int hk_get_stats(hk_context* ctx, hk_frame_stats* out) {
     out->ms_kernel[HK_K_TRACE_RAYS] = ctx->trace_ms;
     out->kernel_launches = ctx->launches;
     out->wide_traversal = (wide_primary(ctx) ? 1u : 0u) | (wide_light(ctx) ? 2u : 0u);
-    out->wide_stack_need = ctx->wide_stack_need;
+    out->wide_stack_need = ctx->sc ? ctx->sc->wide_stack_need : 0u;
     return HK_OK;
 }
 
@@ -1696,16 +1934,17 @@ int hk_upload_state(hk_context* ctx, int which, const void* host, size_t bytes) 
 
 int hk_trace_rays(hk_context* ctx, const hk_ray* rays, size_t n, hk_hit* hits) {
     if (!ctx || (n && (!rays || !hits))) return HK_ERR_INVALID_ARGUMENT;
-    if (!ctx->scene_ready) return set_error(ctx, HK_ERR_NOT_READY, "scene not uploaded");
+    if (!scene_ready(ctx)) return set_error(ctx, HK_ERR_NOT_READY, "scene not uploaded");
     if (n == 0) return HK_OK;
     HK_CUDA(cudaSetDevice(ctx->device));
+    SceneUse use(ctx);
     hk_ray* d_rays = nullptr; hk_hit* d_hits = nullptr;
     HK_CUDA(cudaMalloc(reinterpret_cast<void**>(&d_rays), n * sizeof(hk_ray)));
     cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&d_hits), n * sizeof(hk_hit));
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_rays, rays, n * sizeof(hk_ray), cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) {
         cudaEventRecord(ctx->ev[0], ctx->stream);
-        hk_launch_trace_rays(ctx->scene, d_rays, n, d_hits, wide_light(ctx), ctx->stream);
+        hk_launch_trace_rays(ctx->sc->scene, d_rays, n, d_hits, wide_light(ctx), ctx->stream);
         cudaEventRecord(ctx->ev[1], ctx->stream);
         e = cudaGetLastError();
     }

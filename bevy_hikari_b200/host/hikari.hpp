@@ -225,6 +225,35 @@ struct PrepassNode { static int run(hk_context* ctx, const hk_frame_inputs& in);
 struct LightNode { static int run(hk_context* ctx, const hk_frame_inputs& in); };         // light.rs:590-702
 struct PostProcessNode { static int run(hk_context* ctx, const hk_frame_inputs& in); };   // post_process.rs:1140-1234
 
+// HikariScene: the scene buffers of the render world (MeshMaterialBindGroup, mesh_material/mod.rs:677-681), uploaded and animated
+// once per frame whatever the number of cameras.  create() makes a shared scene (hk_shared_scene) that cameras attach to with
+// HikariPlugin::attach_scene; inside HikariPlugin the same class drives the camera's private scene through its context, so the
+// upload / update logic (and the fallback of update_transforms) exists once.
+class HikariScene {
+public:
+    HikariScene() = default;
+    ~HikariScene();
+    HikariScene(const HikariScene&) = delete;
+    HikariScene& operator=(const HikariScene&) = delete;
+    int create(int cuda_device, void* cuda_stream);         // cuda_stream NULL: the scene creates its own
+    int upload(const MeshMaterialWorld& world);
+    // instance-level buffers only (hk_scene_update_instances): what instance.rs:427-435 rewrites when instances change
+    int update_instances(const MeshMaterialWorld& world);
+    // Animated instances through the device-side rebuild (hk_scene_update_transforms) whenever only transforms changed since the
+    // last prepare_instances; otherwise world.prepare_instances() + hk_scene_update_instances.  *used_device_path says which.
+    int update_transforms(MeshMaterialWorld& world, bool* used_device_path = nullptr);
+    hk_shared_scene* handle() const { return scene_; }      // NULL for a camera's private scene
+    std::string last_error() const;
+
+private:
+    friend class HikariPlugin;
+    hk_shared_scene* scene_ = nullptr;   // a shared scene of its own, or
+    hk_context* ctx_ = nullptr;          // the context whose private scene the hk_scene_* calls write
+    int upload_desc(const hk_scene_desc& d);
+    int update_instances_desc(const hk_scene_desc& d);
+    int update_transforms_arrays(const float* models, const float* previous_models, const float* mesh_aabbs, uint32_t instance_count);
+};
+
 // HikariPlugin: owns the context of one camera, uploads noise + scene, runs the "hikari" sub-graph each frame.
 class HikariPlugin {                          // lib.rs:95-370
 public:
@@ -243,6 +272,11 @@ public:
     // Animated instances through the device-side rebuild (hk_scene_update_transforms) whenever only transforms changed since the
     // last prepare_instances; otherwise world.prepare_instances() + hk_scene_update_instances.  *used_device_path says which.
     int update_transforms(MeshMaterialWorld& world, bool* used_device_path = nullptr);
+    // Render `scene` (a HikariScene after create()) instead of the camera's private scene; the reservoirs are kept.  From then on the
+    // plugin's own upload / update calls are refused: the scene is updated once per frame through `scene` for every camera.
+    int attach_scene(HikariScene& scene);
+    // Back to a private scene (HK_ERR_NOT_READY until the next upload_scene).
+    int detach_scene();
     // One frame of the camera's sub-graph: PREPASS -> LIGHT -> POST_PROCESS (lib.rs:258-365).  Increments the counter
     // first, as frame_counter_system does in PostUpdate (view.rs:89-103).
     int run_frame(const HikariSettings& settings, const ViewInputs& view);
@@ -260,6 +294,7 @@ public:
 
 private:
     hk_context* ctx_ = nullptr;
+    HikariScene scene_;                  // the private scene, through ctx_
 };
 
 }  // namespace hikari

@@ -43,4 +43,20 @@ uint64_t hikari_plugin_frame_counter(hikari_plugin* p) { return P(p)->counter.va
 void hikari_plugin_set_frame_counter(hikari_plugin* p, uint64_t v) { P(p)->counter.value = (size_t)v; }
 void hikari_plugin_set_temporal_upscalers(hikari_plugin* p, int enabled) { P(p)->temporal_upscalers = enabled != 0; }
 
+// ---------------------------------------------------------------------------------------------- shared scene
+static HikariScene* S(hikari_shared_scene* s) { return reinterpret_cast<HikariScene*>(s); }
+hikari_shared_scene* hikari_shared_scene_create(void) { return reinterpret_cast<hikari_shared_scene*>(new HikariScene()); }
+void hikari_shared_scene_destroy(hikari_shared_scene* s) { delete S(s); }
+int hikari_shared_scene_build(hikari_shared_scene* s, int cuda_device, void* cuda_stream) { return S(s)->create(cuda_device, cuda_stream); }
+int hikari_shared_scene_upload(hikari_shared_scene* s, hikari_world* w) { return S(s)->upload(*W(w)); }
+int hikari_shared_scene_update_instances(hikari_shared_scene* s, hikari_world* w) { return S(s)->update_instances(*W(w)); }
+int hikari_shared_scene_update_transforms(hikari_shared_scene* s, hikari_world* w, int* used_device_path) {
+    bool used = false;
+    int rc = S(s)->update_transforms(*W(w), &used);
+    if (used_device_path) *used_device_path = used ? 1 : 0;
+    return rc;
+}
+hk_shared_scene* hikari_shared_scene_handle(hikari_shared_scene* s) { return S(s)->handle(); }
+int hikari_plugin_attach_scene(hikari_plugin* p, hikari_shared_scene* s) { return s ? P(p)->attach_scene(*S(s)) : P(p)->detach_scene(); }
+
 }  // extern "C"

@@ -201,6 +201,43 @@ int hk_scene_update_instances(hk_context* ctx, const hk_scene_desc* scene);
  * costs one small read-back and a stream synchronisation; otherwise the call never waits for the device. */
 int hk_scene_update_transforms(hk_context* ctx, const float* models, const float* previous_models, const float* mesh_aabbs,
                                uint32_t instance_count);
+/* Shared scenes: several cameras render ONE scene, uploaded and animated once per frame.  The reference keeps one set of scene
+ * buffers for the whole render world (MeshMaterialBindGroup, src/mesh_material/mod.rs:677-681) that every camera's LightNode binds
+ * (src/light.rs:641-642); only reservoirs and textures are per camera (ReservoirCache, src/light.rs:69,307-383).  Split screen, a
+ * minimap or a render-to-texture mirror are one hk_shared_scene and one hk_context per view.
+ *
+ * hk_scene_upload(ctx, ..) gives a context a PRIVATE scene on the context's own stream (what every caller without shared scenes
+ * uses, unchanged); hk_scene_update_* / hk_scene_readback / hk_scene_buffer_bytes then work on whatever scene the context has.  A
+ * shared scene is created by hk_shared_scene_create — on `cuda_stream`, or on a stream of its own when NULL — uploaded and updated
+ * through its handle with the same rules as the hk_scene_* calls above, and attached to any number of contexts of the same device:
+ *   - hk_context_attach_scene(ctx, s): the context renders `s` from its next frame on.  A context of another device than `s` is
+ *     refused (HK_ERR_INVALID_ARGUMENT).  Attaching keeps the context's reservoirs and planes (a scene change does not reset the
+ *     reference's temporal state either); it drops the context's previous scene (a private one is freed).  NULL detaches: the
+ *     frame calls then return HK_ERR_NOT_READY, as they do on a context whose scene has not been uploaded.
+ *   - hk_scene_upload / hk_scene_update_* on a context whose scene is shared return HK_ERR_INVALID_ARGUMENT and leave the scene
+ *     untouched: updates go through the hk_shared_scene handle.
+ *   - hk_shared_scene_destroy drops the caller's handle; the scene's memory goes with the last attached context (detach or
+ *     hk_context_destroy), so cameras keep rendering after the handle is gone.
+ *   - Stream order: a scene update first makes the scene's stream wait until every attached context on another stream has issued
+ *     the last launch of its last frame call that reads the scene (hk_prepass_run, hk_light_run, hk_run_pass, hk_trace_rays,
+ *     hk_render_frame), then rewrites the buffers; such a context's next frame waits for the update on the device.  No buffer a
+ *     camera may still read is freed before that camera has finished with it.  Nothing is waited for on the host except where the
+ *     hk_scene_* calls already synchronise (full uploads, instance updates, the 4-wide TLAS read-back of hk_scene_update_transforms,
+ *     which with a shared scene also waits for the cameras' frames in flight).  A context on the scene's own stream records and
+ *     waits for nothing: stream order already holds.
+ *   - hk_shared_scene_update_transforms re-derives the 4-wide TLAS when ANY attached context walks the 4-wide trees
+ *     (HK_TUNE_WIDE_TRAVERSAL stays a per-context setting).
+ *   - Threading: a scene and every context attached to it are driven from one thread at a time (Bevy 0.9's render graph does this).
+ * Errors of the hk_shared_scene_* calls are reported by hk_shared_scene_last_error(s) (s = NULL: the last failed create). */
+typedef struct hk_shared_scene hk_shared_scene;
+int hk_shared_scene_create(hk_shared_scene** out, int cuda_device, void* cuda_stream);   /* NULL stream: the scene creates its own */
+void hk_shared_scene_destroy(hk_shared_scene* s);       /* drops the caller's reference; memory goes with the last attached context */
+int hk_shared_scene_upload(hk_shared_scene* s, const hk_scene_desc* scene);
+int hk_shared_scene_update_instances(hk_shared_scene* s, const hk_scene_desc* scene);
+int hk_shared_scene_update_transforms(hk_shared_scene* s, const float* models, const float* previous_models,
+                                      const float* mesh_aabbs, uint32_t instance_count);
+const char* hk_shared_scene_last_error(hk_shared_scene* s);
+int hk_context_attach_scene(hk_context* ctx, hk_shared_scene* s);   /* NULL detaches; frees a private scene */
 /* Test / debugging aid: the per-frame scene buffers as they are on the device, in the layouts of hk_layout.h. */
 enum { HK_SCENE_INSTANCES = 0, HK_SCENE_INSTANCE_NODES = 1, HK_SCENE_EMISSIVES = 2, HK_SCENE_EMISSIVE_NODES = 3,
        HK_SCENE_PREVIOUS_MODELS = 4 /* 64 B per instance; empty when nothing moved */, HK_SCENE_INSTANCE_MOVED = 5 /* uint32 per instance */ };

@@ -114,6 +114,22 @@ void hikari_plugin_set_frame_counter(hikari_plugin* p, uint64_t v);
 /* 1 = run_frame continues past tone mapping with smaa_tu4x / taa_jasmine as the settings select (post_process.rs:1236-1277) */
 void hikari_plugin_set_temporal_upscalers(hikari_plugin* p, int enabled);
 
+/* HikariScene: one scene, uploaded and animated once per frame, that several cameras render (hk_shared_scene, hikari_b200.h).
+ * build creates it on `cuda_stream` (NULL: a stream of its own); upload / update_instances / update_transforms are those of
+ * hikari_plugin_*, for every attached camera at once.  Errors: hk_shared_scene_last_error(hikari_shared_scene_handle(s)).
+ * destroy drops the handle; the scene lives on while a camera renders it. */
+typedef struct hikari_shared_scene hikari_shared_scene;
+hikari_shared_scene* hikari_shared_scene_create(void);
+void hikari_shared_scene_destroy(hikari_shared_scene* s);
+int hikari_shared_scene_build(hikari_shared_scene* s, int cuda_device, void* cuda_stream);
+int hikari_shared_scene_upload(hikari_shared_scene* s, hikari_world* w);
+int hikari_shared_scene_update_instances(hikari_shared_scene* s, hikari_world* w);
+int hikari_shared_scene_update_transforms(hikari_shared_scene* s, hikari_world* w, int* used_device_path);
+hk_shared_scene* hikari_shared_scene_handle(hikari_shared_scene* s);
+/* the camera renders `s` from its next frame on, keeping its reservoirs (hk_context_attach_scene); its own upload / update calls
+ * are refused while it does.  s = NULL: back to a private scene, HK_ERR_NOT_READY until hikari_plugin_upload_scene. */
+int hikari_plugin_attach_scene(hikari_plugin* p, hikari_shared_scene* s);
+
 #ifdef __cplusplus
 }
 #endif

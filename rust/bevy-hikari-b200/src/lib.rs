@@ -19,6 +19,32 @@ use bevy::{
 use bevy_hikari::{prelude::*, view::{FrameUniform, PreviousViewUniform}};
 use hikari_b200_sys as ffi;
 
+/// The scene buffers of the render world, ONE for every camera: the reference's `MeshMaterialBindGroup` is a single resource
+/// (src/mesh_material/mod.rs:677-681) that every camera's `LightNode` binds (src/light.rs:641-642).  Uploaded and animated once per
+/// frame; each camera's context attaches to it (include/hikari_b200.h: hk_shared_scene).  Dropping it drops the handle only: the
+/// device memory goes with the last camera context that renders it.
+#[derive(Resource)]
+pub struct HikariB200Scene(pub *mut ffi::hk_shared_scene);
+unsafe impl Send for HikariB200Scene {}
+unsafe impl Sync for HikariB200Scene {}
+
+impl FromWorld for HikariB200Scene {
+    fn from_world(_world: &mut World) -> Self {
+        let mut scene = std::ptr::null_mut();
+        // a stream of its own: cameras on other streams are ordered against it by the library
+        if unsafe { ffi::hk_shared_scene_create(&mut scene, 0, std::ptr::null_mut()) } != ffi::HK_OK {
+            error!("hk_shared_scene_create: {}", scene_error(std::ptr::null_mut()));
+        }
+        HikariB200Scene(scene)
+    }
+}
+
+impl Drop for HikariB200Scene {
+    fn drop(&mut self) {
+        unsafe { ffi::hk_shared_scene_destroy(self.0) }
+    }
+}
+
 /// One `hk_context` per camera entity (what `ReservoirCache` + the texture caches are in the reference, src/light.rs:307-383).
 #[derive(Component)]
 pub struct HikariB200Context(pub *mut ffi::hk_context);
@@ -31,9 +57,11 @@ impl Drop for HikariB200Context {
     }
 }
 
-/// `prepare_light_textures` / `prepass_textures_system` / `prepare_post_process_textures` collapse into create-or-resize.
+/// `prepare_light_textures` / `prepass_textures_system` / `prepare_post_process_textures` collapse into create-or-resize; a new
+/// camera's context is attached to the render world's one scene (only reservoirs and textures are per camera, src/light.rs:69).
 pub fn prepare_contexts(
     mut commands: Commands,
+    scene: Res<HikariB200Scene>,
     cameras: Query<(Entity, &ExtractedCamera, Option<&HikariB200Context>), With<HikariSettings>>,
 ) {
     for (entity, camera, context) in &cameras {
@@ -46,14 +74,21 @@ pub fn prepare_contexts(
             None => {
                 let mut ctx = std::ptr::null_mut();
                 let rc = unsafe { ffi::hk_context_create(&mut ctx, 0, size.x, size.y, 0, size.y, std::ptr::null_mut()) };
-                if rc == ffi::HK_OK {
-                    commands.entity(entity).insert(HikariB200Context(ctx));
-                } else {
+                if rc != ffi::HK_OK {
                     error!("hk_context_create: {}", last_error(std::ptr::null_mut()));
+                    continue;
                 }
+                if unsafe { ffi::hk_context_attach_scene(ctx, scene.0) } != ffi::HK_OK {
+                    error!("hk_context_attach_scene: {}", last_error(ctx));
+                }
+                commands.entity(entity).insert(HikariB200Context(ctx));
             }
         }
     }
+}
+
+fn scene_error(scene: *mut ffi::hk_shared_scene) -> String {
+    unsafe { CStr::from_ptr(ffi::hk_shared_scene_last_error(scene)) }.to_string_lossy().into_owned()
 }
 
 fn last_error(ctx: *mut ffi::hk_context) -> String {
@@ -145,34 +180,35 @@ hikari_node!(PrepassNode, ffi::hk_prepass_run, "Replaces `PrepassNode::run` (src
 hikari_node!(LightNode, ffi::hk_light_run, "Replaces `LightNode::run` (src/light.rs:590-702): albedo, both direct passes, indirect, spatial reuse.");
 hikari_node!(PostProcessNode, ffi::hk_post_process_run, "Replaces `PostProcessNode::run` (src/post_process.rs:1140-1311): denoise, tone mapping, SMAA TU4x / TAA / FSR1.");
 
-/// Hands the nine storage buffers of bind group 2 (src/mesh_material/mod.rs:684-808) to the device whenever any of them changed.
+/// Hands the nine storage buffers of bind group 2 (src/mesh_material/mod.rs:684-808) to the device whenever any of them changed —
+/// once per frame for every camera, into the shared scene.
 /// The encase byte images are `#[repr(C)]`-compatible with include/hk_layout.h (static_asserts there, size assertions in the -sys crate).
-pub fn upload_scene(ctx: &HikariB200Context, scene: &ffi::hk_scene_desc, instances_only: bool) {
+pub fn upload_scene(scene: &HikariB200Scene, desc: &ffi::hk_scene_desc, instances_only: bool) {
     let rc = unsafe {
-        if instances_only { ffi::hk_scene_update_instances(ctx.0, scene) } else { ffi::hk_scene_upload(ctx.0, scene) }
+        if instances_only { ffi::hk_shared_scene_update_instances(scene.0, desc) } else { ffi::hk_shared_scene_upload(scene.0, desc) }
     };
     if rc != ffi::HK_OK {
-        error!("scene upload: {}", last_error(ctx.0));
+        error!("scene upload: {}", scene_error(scene.0));
     }
 }
 
 /// Frames on which only `GlobalTransform`s changed (the common case of an animated scene): the per-frame half of the scene —
-/// instance AABBs and matrices, TLAS, emissives, emissive BVH — is rebuilt ON THE DEVICE from one matrix per instance
-/// (include/hikari_b200.h: hk_scene_update_transforms; replaces the CPU work of src/mesh_material/instance.rs:352-437).
+/// instance AABBs and matrices, TLAS, emissives, emissive BVH — is rebuilt ON THE DEVICE from one matrix per instance, once for
+/// every camera (include/hikari_b200.h: hk_shared_scene_update_transforms; replaces the CPU work of src/mesh_material/instance.rs:352-437).
 /// `models` / `previous_models`: `GlobalTransform::compute_matrix().to_cols_array()` of every instance in instance order and its
 /// `GlobalTransformQueue[1]`; `mesh_aabbs`: `[center.x, center.y, center.z, half.x, half.y, half.z]` of each instance's mesh `Aabb`.
 /// The caller keeps the reference's conditions for the full path (instance set changed, or an emissive's scale left its cached alias
 /// table's +-0.01 range, instance.rs:385-397) and calls `upload_scene(.., instances_only = true)` then.
-pub fn update_transforms(ctx: &HikariB200Context, models: &[[f32; 16]], previous_models: Option<&[[f32; 16]]>, mesh_aabbs: &[[f32; 6]]) -> bool {
+pub fn update_transforms(scene: &HikariB200Scene, models: &[[f32; 16]], previous_models: Option<&[[f32; 16]]>, mesh_aabbs: &[[f32; 6]]) -> bool {
     debug_assert!(models.len() == mesh_aabbs.len() && previous_models.map_or(true, |p| p.len() == models.len()));
     let rc = unsafe {
-        ffi::hk_scene_update_transforms(ctx.0, models.as_ptr() as *const f32, previous_models.map_or(std::ptr::null(), |p| p.as_ptr() as *const f32),
-                                        mesh_aabbs.as_ptr() as *const f32, models.len() as u32)
+        ffi::hk_shared_scene_update_transforms(scene.0, models.as_ptr() as *const f32, previous_models.map_or(std::ptr::null(), |p| p.as_ptr() as *const f32),
+                                               mesh_aabbs.as_ptr() as *const f32, models.len() as u32)
     };
     match rc {
         ffi::HK_OK => true,
         ffi::HK_ERR_UNSUPPORTED => false,      // a TLAS that is not in bvh 0.7.1's layout: keep the host path
-        _ => { error!("hk_scene_update_transforms: {}", last_error(ctx.0)); false }
+        _ => { error!("hk_shared_scene_update_transforms: {}", scene_error(scene.0)); false }
     }
 }
 
