@@ -64,6 +64,7 @@ struct hk_shared_scene {
     std::vector<void*> scene_allocations;  // scene buffers: meshes, BLAS nodes, materials, textures
     struct DevBuf { void* p = nullptr; size_t cap = 0; } ibuf[20];  // scene buffers rewritten by hk_scene_update_instances (grow-only);
                                                                     // 14-19: staging + scratch of hk_scene_update_transforms
+                                                                    // (15: DeviceScene::wide_state, 16: kc_build_wide_tlas's scratch)
     // hk_scene_update_transforms: what the last full upload fixed, and pinned staging (two slots, so that the host never waits for
     // the copy of the previous call unless it is two calls behind)
     uint32_t scene_instance_count = 0, scene_emissive_count = 0;
@@ -75,8 +76,11 @@ struct hk_shared_scene {
     std::vector<std::array<uint32_t, 3>> wide_mesh_keys;    // (node_offset, node_count, primitive) in first-use order
     std::vector<WideMesh> wide_meshes;                      // parallel to wide_mesh_keys
     uint32_t wide_blas_node_count = 0;
-    uint32_t wide_tlas_node_count = 0;
-    uint32_t wide_stack_need = 0;
+    uint32_t wide_tlas_node_count = 0;     // of the last host derivation (upload / instance update): wide_primary's size rule
+    uint32_t wide_stack_need = 0;          // of the last host derivation
+    bool wide_blas_ok = false;             // every instance's mesh has a 4-wide tree ...
+    uint32_t wide_blas_need = 0;           // ... and the deepest of them needs this much stack
+    bool wide_on_device = false;           // the 4-wide TLAS was last derived on the device: its verdict is in ibuf[15] only
     bool mesh_boxes_match = false;         // BLAS half of DeviceScene::leaf_boxes_match
     uint32_t scene_material_count = 0, scene_asset_node_count = 0, scene_primitive_count = 0, scene_vertex_count = 0, scene_texture_count = 0;
     std::vector<hk_node> host_asset_nodes;                 // copy of the uploaded BLAS records: index validation of later instance updates
@@ -579,31 +583,56 @@ static cudaError_t upload_into(hk_shared_scene* sc, hk_shared_scene::DevBuf& b, 
     return e;
 }
 
+// grow-only device scratch
+static cudaError_t ensure_buf(hk_shared_scene* sc, hk_shared_scene::DevBuf& b, size_t bytes) {
+    const size_t need = bytes + 64;
+    if (b.cap >= need) return cudaSuccess;
+    if (b.p) { scene_before_free(sc); cudaFree(b.p); }
+    b.p = nullptr; b.cap = 0;
+    const size_t cap = need + need / 2;
+    cudaError_t e = cudaMalloc(&b.p, cap);
+    if (e == cudaSuccess) b.cap = cap;
+    return e;
+}
+
 // The 4-wide tree over the instances (the half of upload_wide that every instance update repeats) from the flat TLAS in `nodes`
 // (host memory) and the instances' boxes (6 floats each, or null when the navigators carry them by construction); the meshes' trees
 // and sc->wide_mesh_of are those of the last upload_wide.
 static int upload_wide_tlas(hk_shared_scene* sc, const hk_node* nodes, uint32_t node_count, uint32_t instance_count, const float* instance_box,
                             DeviceScene& d) {
     d.wide_ready = 0u; d.wide_tlas_root = WIDE_EMPTY;
+    sc->wide_on_device = false;
     hkw::WideTree tlas = hkw::build_wide(nodes, node_count, instance_count, instance_box);
-    bool ok = tlas.ok && sc->wide_mesh_of.size() == instance_count;
+    bool blas_ok = sc->wide_mesh_of.size() == instance_count;
     uint32_t blas_need = 0;
     std::vector<uint2> entry(instance_count);
     for (uint32_t i = 0; i < instance_count && sc->wide_mesh_of.size() == instance_count; ++i) {
         const hk_shared_scene::WideMesh& m = sc->wide_meshes[sc->wide_mesh_of[i]];
-        ok = ok && m.ok;
+        blas_ok = blas_ok && m.ok;
         entry[i] = make_uint2(m.base, m.root);
         blas_need = std::max(blas_need, m.need);
     }
+    const bool ok = tlas.ok && blas_ok;
+    sc->wide_blas_ok = blas_ok;
+    sc->wide_blas_need = blas_need;
     if (!tlas.ok) { tlas.nodes.clear(); tlas.rank.assign(instance_count, 0u); }
     sc->wide_tlas_node_count = (uint32_t)tlas.nodes.size();
+    // hk_scene_update_transforms re-derives the tree into the same buffers on the device: sized here for the largest tree over these
+    // instances (n - 1 nodes, n ranks) with its scratch, so that the update allocates nothing
+    const size_t max_nodes = instance_count > 1u ? instance_count - 1u : 1u;
+    HK_SCUDA(ensure_buf(sc, sc->ibuf[9], sizeof(hk_wide_node) * max_nodes));
+    HK_SCUDA(ensure_buf(sc, sc->ibuf[12], sizeof(uint32_t) * (size_t)instance_count));
+    HK_SCUDA(ensure_buf(sc, sc->ibuf[16], hk_wide_tlas_scratch_bytes(instance_count)));
     HK_SCUDA(upload_into(sc, sc->ibuf[9], &d.wide_tlas, tlas.nodes.data(), tlas.nodes.size()));
     HK_SCUDA(upload_into(sc, sc->ibuf[11], &d.wide_instance, entry.data(), entry.size()));
     HK_SCUDA(upload_into(sc, sc->ibuf[12], &d.wide_instance_rank, tlas.rank.data(), tlas.rank.size()));
-    HK_SCUDA(cudaStreamSynchronize(sc->stream));
     // pending TLAS siblings + the BLAS marker + pending BLAS siblings, and the three pushes a node step makes before it pops
     sc->wide_stack_need = tlas.stack_need + 1u + blas_need + 3u;
-    if (ok && sc->wide_stack_need <= (uint32_t)HK_WIDE_STACK) {
+    const bool ready = ok && sc->wide_stack_need <= (uint32_t)HK_WIDE_STACK;
+    const uint32_t state[3] = {ready ? 1u : 0u, sc->wide_stack_need, sc->wide_tlas_node_count};
+    HK_SCUDA(upload_into(sc, sc->ibuf[15], &d.wide_state, state, 3));
+    HK_SCUDA(cudaStreamSynchronize(sc->stream));
+    if (ready) {
         d.wide_tlas_root = tlas.root;
         d.wide_ready = 1u;
     }
@@ -915,17 +944,6 @@ extern "C" {      // (defined with the scheduling below)
 static bool wide_primary(const hk_context* ctx);
 static bool wide_light(const hk_context* ctx);
 }
-// grow-only device scratch
-static cudaError_t ensure_buf(hk_shared_scene* sc, hk_shared_scene::DevBuf& b, size_t bytes) {
-    const size_t need = bytes + 64;
-    if (b.cap >= need) return cudaSuccess;
-    if (b.p) { scene_before_free(sc); cudaFree(b.p); }
-    b.p = nullptr; b.cap = 0;
-    const size_t cap = need + need / 2;
-    cudaError_t e = cudaMalloc(&b.p, cap);
-    if (e == cudaSuccess) b.cap = cap;
-    return e;
-}
 
 // SURVEY 8(f) rank 2 — the per-frame half of the scene rebuilt on the device (kernels_scene.cu) from the model matrices alone.
 static int scene_update_transforms(hk_shared_scene* sc, const float* models, const float* previous_models, const float* mesh_aabbs,
@@ -983,36 +1001,63 @@ static int scene_update_transforms(hk_shared_scene* sc, const float* models, con
                               static_cast<float4*>(sc->ibuf[5].p), static_cast<uint32_t*>(sc->ibuf[6].p), box_lo, box_hi, sc->stream);
     hk_launch_build_flat_bvh(n, box_lo, box_hi, sc->ibuf[19].p, static_cast<hk_node*>(sc->ibuf[2].p),
                              reinterpret_cast<uint8_t*>(instances) + offsetof(hk_instance, node_index), (uint32_t)sizeof(hk_instance), sc->stream);
+    bool wide = false;          // the 4-wide TLAS is re-derived when any attached camera walks the wide trees
+    for (const hk_context* c : sc->attached) wide = wide || wide_primary(c) || wide_light(c);
+    if (wide) {
+        // image-exact traversal mode in use: its 4-wide TLAS is derived on the device from the records just built, into the buffers
+        // upload_wide_tlas sized for these instances (leaf navigators = instance boxes, as built).  Whether it fits the walk's stack
+        // is known only there: the WIDE launches read the verdict (DeviceScene::wide_state), the host never waits for it
+        hk_launch_build_wide_tlas(n, static_cast<const hk_node*>(sc->ibuf[2].p), sc->wide_blas_ok, 1u + sc->wide_blas_need + 3u, sc->ibuf[16].p,
+                                  static_cast<hk_wide_node*>(sc->ibuf[9].p), static_cast<uint32_t*>(sc->ibuf[12].p),
+                                  static_cast<uint32_t*>(sc->ibuf[15].p), sc->stream);
+    }
     if (ne) {
         hk_launch_scene_emissives(ne, emissives, instances, d.materials, d.primitives, d.vertices, box_lo, box_hi, sc->stream);
         hk_launch_build_flat_bvh(ne, box_lo, box_hi, sc->ibuf[19].p, static_cast<hk_node*>(sc->ibuf[3].p),
                                  reinterpret_cast<uint8_t*>(emissives) + offsetof(hk_emissive, node_index), (uint32_t)sizeof(hk_emissive), sc->stream);
     }
     HK_SCUDA(cudaGetLastError());
-    *launches = ne ? 4u : 2u;
+    *launches = (ne ? 4u : 2u) + (wide ? 1u : 0u);
     d.previous_models = static_cast<const float4*>(sc->ibuf[5].p);
     d.instance_moved = static_cast<const uint32_t*>(sc->ibuf[6].p);
     d.leaf_boxes_match = sc->mesh_boxes_match ? 1u : 0u;       // every navigator carries its instance's own box by construction
     d.wide_ready = 0u; d.wide_tlas_root = WIDE_EMPTY;
-    bool wide = false;          // the 4-wide TLAS is re-derived when any attached camera walks the wide trees
-    for (const hk_context* c : sc->attached) wide = wide || wide_primary(c) || wide_light(c);
     if (wide) {
-        // image-exact traversal mode in use: its 4-wide TLAS is derived on the host from the records just built (one small read-back;
-        // scenes that walk the reference's arrays never reach this and never synchronise)
-        std::vector<hk_node> nodes(tlas_records);
-        HK_SCUDA(cudaMemcpyAsync(nodes.data(), sc->ibuf[2].p, sizeof(hk_node) * (size_t)tlas_records, cudaMemcpyDeviceToHost, sc->stream));
-        HK_SCUDA(cudaStreamSynchronize(sc->stream));
-        int rc = upload_wide_tlas(sc, nodes.data(), tlas_records, n, nullptr, d);     // leaf navigators = instance boxes, as built
-        if (rc != HK_OK) return rc;
+        d.wide_tlas = static_cast<const hk_wide_node*>(sc->ibuf[9].p);
+        d.wide_instance_rank = static_cast<const uint32_t*>(sc->ibuf[12].p);
+        d.wide_state = static_cast<const uint32_t*>(sc->ibuf[15].p);
+        d.wide_tlas_root = n == 1u ? WIDE_LEAF : 0u;      // what build_wide returns for bvh 0.7.1's layout
+        d.wide_ready = sc->wide_blas_ok ? 1u : 0u;         // the meshes' half; the TLAS's half is wide_state[0]
+        sc->wide_on_device = true;
     }
     sc->scene = d;
     return HK_OK;
 }
 
+// {ready, stack need, TLAS node count} of the scene's 4-wide TLAS.  After a derivation on the device they exist only there
+// and are read back: a query (hk_get_stats, hk_scene_readback), not a frame call, so it may wait for the scene's stream.
+static cudaError_t wide_tlas_state(hk_shared_scene* sc, uint32_t out[3]) {
+    if (!sc->wide_on_device) {
+        out[0] = sc->scene.wide_ready; out[1] = sc->wide_stack_need; out[2] = sc->wide_tlas_node_count;
+        return cudaSuccess;
+    }
+    cudaError_t e = cudaMemcpyAsync(out, sc->ibuf[15].p, 3u * sizeof(uint32_t), cudaMemcpyDeviceToHost, sc->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(sc->stream);
+    return e;
+}
+
 // Test / debugging aid: the per-frame scene buffers as they are on the device (what hk_scene_update_transforms built in place).
-static bool scene_buffer(const hk_shared_scene* sc, int which, const void** src, size_t* have) {
+static bool scene_buffer(hk_shared_scene* sc, int which, const void** src, size_t* have) {
     const DeviceScene& d = sc->scene;
     switch (which) {
+        case HK_SCENE_WIDE_TLAS: {
+            uint32_t state[3] = {0u, 0u, 0u};
+            if (wide_tlas_state(sc, state) != cudaSuccess) return false;
+            *src = d.wide_tlas; *have = d.wide_tlas ? sizeof(hk_wide_node) * (size_t)state[2] : 0u;
+            return true;
+        }
+        case HK_SCENE_WIDE_INSTANCE_RANK:
+            *src = d.wide_instance_rank; *have = d.wide_instance_rank ? 4u * (size_t)sc->scene_instance_count : 0u; return true;
         case HK_SCENE_INSTANCES: *src = d.instances; *have = sizeof(hk_instance) * (size_t)sc->scene_instance_count; return true;
         case HK_SCENE_INSTANCE_NODES: *src = d.instance_nodes; *have = sizeof(hk_node) * (size_t)d.instance_node_count; return true;
         case HK_SCENE_EMISSIVES: *src = d.emissives; *have = sizeof(hk_emissive) * (size_t)sc->scene_emissive_count; return true;
@@ -1556,6 +1601,12 @@ int hk_get_stats(hk_context* ctx, hk_frame_stats* out) {
     out->kernel_launches = ctx->launches;
     out->wide_traversal = (wide_primary(ctx) ? 1u : 0u) | (wide_light(ctx) ? 2u : 0u);
     out->wide_stack_need = ctx->sc ? ctx->sc->wide_stack_need : 0u;
+    if (ctx->sc && ctx->sc->wide_on_device) {      // the last 4-wide TLAS was derived on the device: so are its verdict and stack need
+        uint32_t state[3];
+        HK_CUDA(wide_tlas_state(ctx->sc, state));
+        if (!state[0]) out->wide_traversal = 0u;
+        out->wide_stack_need = state[1];
+    }
     return HK_OK;
 }
 

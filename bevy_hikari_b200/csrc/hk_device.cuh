@@ -97,8 +97,15 @@ struct DeviceScene {
     const uint32_t* wide_instance_rank;      // per instance: position of its leaf in instance_nodes (array order = the reference's visit order)
     const uint32_t* wide_primitive_rank;     // per primitive: position of its leaf in its mesh's asset_nodes range
     uint32_t wide_tlas_root;
-    uint32_t wide_ready;                     // 1 = every tree could be derived and fits the walk's stack
+    uint32_t wide_ready;                     // 1 = every tree could be derived (and, after a host derivation, fits the walk's stack)
+    // {ready, stack need, TLAS node count} of the 4-wide TLAS on the device: written by the host derivation and by
+    // kc_build_wide_tlas.  Whether a TLAS derived on the device fits the walk's stack is known only here, so the WIDE launches read
+    // state[0] and take the reference's walk when it is 0
+    const uint32_t* wide_state;
 };
+
+// WIDE launches: does the 4-wide TLAS this launch sees fit the walk's stack?  One word, the same for every thread
+__device__ __forceinline__ bool wide_tlas_ready(const DeviceScene& sc) { return __ldg(sc.wide_state) != 0u; }
 
 struct ReservoirPlanes {  // one PackedReservoir buffer as 4 planes
     uint4* q[4];
@@ -817,12 +824,15 @@ static __device__ HK_INL_SELECT LightCandidate select_light_candidate(const Devi
             if (COUNT_RAYS) blas_rays += 1u;
             Ray r;
             instance_ray(einst, ray, r);
+            bool walked = false;        // a launch whose 4-wide TLAS does not fit the stack walks every tree the reference's way
             if constexpr (WIDE) {
-                hit = wide_walk<true>(sc, r, F32_MAX, 0.0f, DONT_EXCLUDE, cand.emissive_instance);
-                found = hit.primitive_index != U32_MAX;
-            } else {
-                found = traverse_bottom(sc, hit, r, mesh.y, mesh.z, mesh.w, 0.0f);
+                if (wide_tlas_ready(sc)) {
+                    hit = wide_walk<true>(sc, r, F32_MAX, 0.0f, DONT_EXCLUDE, cand.emissive_instance);
+                    found = hit.primitive_index != U32_MAX;
+                    walked = true;
+                }
             }
+            if (!walked) found = traverse_bottom(sc, hit, r, mesh.y, mesh.z, mesh.w, 0.0f);
         }
         if (found) {
             hit.instance_index = e2.x;

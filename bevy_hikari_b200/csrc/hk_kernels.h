@@ -45,5 +45,11 @@ void hk_launch_scene_instances(uint32_t n, const float4* models, const float4* p
 void hk_launch_build_flat_bvh(uint32_t n, const float4* box_lo, const float4* box_hi, void* scratch, hk_node* out, void* index_base,
                               uint32_t index_stride, cudaStream_t st);
 size_t hk_scene_bvh_scratch_bytes(uint32_t n);
+// the 4-wide TLAS (hk_wide.cuh) of the flat TLAS flat[0 .. 3n-2) over n instances, as wide_build.h derives it: at most n - 1 nodes,
+// n ranks, and state = {ready, stack need of the whole walk, node count} where ready = blas_ok && the tree could be derived
+// && its need + base_need <= HK_WIDE_STACK.  `scratch`: hk_wide_tlas_scratch_bytes(n) bytes.
+void hk_launch_build_wide_tlas(uint32_t n, const hk_node* flat, bool blas_ok, uint32_t base_need, void* scratch, hkd::hk_wide_node* nodes,
+                               uint32_t* rank, uint32_t* state, cudaStream_t st);
+size_t hk_wide_tlas_scratch_bytes(uint32_t n);
 void hk_launch_scene_emissives(uint32_t ne, hk_emissive* emissives, const hk_instance* instances, const hk_material* materials,
                                const hk_primitive* primitives, const hk_vertex* vertices, float4* box_lo, float4* box_hi, cudaStream_t st);

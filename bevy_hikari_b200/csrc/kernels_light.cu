@@ -35,11 +35,14 @@ __device__ __forceinline__ void flush_counters(const KParams& P, uint32_t primar
     }
 }
 
-// traverse_top in the launch's traversal mode: WIDE = the image-exact 4-wide walk (hk_wide.cuh), else the reference's fixed-order walk
+// traverse_top in the launch's traversal mode: WIDE = the image-exact 4-wide walk (hk_wide.cuh) when the device's 4-wide TLAS fits the
+// walk's stack, else the reference's fixed-order walk
 template <bool WIDE>
 __device__ __forceinline__ Hit trace_top(const DeviceScene& sc, const Ray& ray, float max_distance, float early_distance, uint32_t exclude_instance) {
-    if constexpr (WIDE) return wide_walk<false>(sc, ray, max_distance, early_distance, exclude_instance, 0u);
-    else return traverse_top(sc, ray, max_distance, early_distance, exclude_instance);
+    if constexpr (WIDE) {
+        if (wide_tlas_ready(sc)) return wide_walk<false>(sc, ray, max_distance, early_distance, exclude_instance, 0u);
+    }
+    return traverse_top(sc, ray, max_distance, early_distance, exclude_instance);
 }
 
 __device__ __forceinline__ mat4 load_mat4(const float* m) {

@@ -18,10 +18,15 @@
 //     counting sort;
 //   * a node's place in the flat array follows from how many tree nodes and leaves precede it in pre-order: a subtree of m shapes
 //     has 2m - 1 tree nodes and writes 3m - 1 records, so both children's places are known when the parent splits.
+// When a camera walks the 4-wide trees (HK_TUNE_WIDE_TRAVERSAL), one more kernel follows the TLAS build:
+//   kc_build_wide_tlas   one CTA: the image-exact traversal mode's 4-wide TLAS (hk_wide.cuh) from the flat TLAS just built, byte for
+//                        byte what wide_build.h derives on the host at upload, and the verdict "fits the walk's stack"
+//                        (tests/test_gpu_wide_tlas_device.py holds it to the host derivation)
 // What this path does NOT rebuild: alias tables (their cache rule — rebuild when the scale moved by more than 0.01,
 // instance.rs:385-397 — is the caller's to check: hikari::MeshMaterialWorld::prepare_instance_transforms) and anything that changes
 // the SET of instances, meshes or materials; those go through hk_scene_update_instances / hk_scene_upload.
 #include "hk_device.cuh"
+#include "hk_wide.cuh"
 #include "hk_kernels.h"
 
 namespace hkd {
@@ -423,6 +428,263 @@ __global__ void __launch_bounds__(128) kc_scene_emissives(uint32_t ne, hk_emissi
     }
 }
 
+// ------------------------------------------------------------------------------------------------ 4-wide TLAS
+// hkw::build_wide(flat, 3n - 2, n, nullptr) (wide_build.h) restated for one CTA, so that hk_scene_update_transforms leaves the 4-wide
+// TLAS on the device instead of reading the flat one back.  The same tree, node for node:
+//   parse     one thread per record: a navigator's branches are the chain of exit links that starts behind it (Parser::range), checked
+//             as the host checks them — links that nest, at most four branches, leaf branches of two records naming a shape < n,
+//             navigator boxes that enclose their branches' boxes, no deeper than the host's recursion limit — and a leaf's rank is
+//             the number of leaf records before it (block-wide scan); a shape named by two leaves fails
+//   collapse  level by level, one thread per wide node: open the branch with the largest half_area while the result still fits in
+//             four, the first of equal areas (detail::emit); the branches left that are not leaves are the next level's wide nodes
+//   sizes     bottom-up: wide subtree sizes and stack needs, need = max((k - 1) + the child's need)
+//   write     top-down: pre-order indices (a node before its children, children in order) and the 128-byte nodes, empty_node padding
+// state = {ready, stack need of the whole walk, node count}: ready = blas_ok && tlas ok && need <= HK_WIDE_STACK, where
+// need = the TLAS's need + base_need (the BLAS marker, the meshes' need and the slack, context.cu upload_wide_tlas).  A tree the host
+// would refuse leaves node count 0 and every rank 0, as upload_wide_tlas does.
+constexpr uint32_t WB_OK = 8u, WB_LEAF = 16u;      // rec_meta: branch count (0-4) | WB_OK | WB_LEAF (a leaf branch: rec_kids.x = shape)
+constexpr uint32_t WB_MAX_DEPTH = 200u;            // Parser::range refuses a deeper recursion
+
+struct WideScratch {
+    uint32_t* rec_meta;      // per record, and the top-level range at index `count`
+    uint4* rec_kids;         // per record: the records of its branches, or .x = the shape of a leaf branch
+    uint32_t* wn_bin;        // per wide node, in level order: its record (`count` = the top-level range)
+    uint32_t* wn_depth;      // depth of Parser::range at which its branches are found
+    uint32_t* wn_k;          // branches after collapsing
+    uint4* wn_kids;          // their records
+    uint4* wn_child;         // per branch: slot of its wide node, or WIDE_EMPTY (a leaf)
+    uint32_t *wn_size, *wn_need, *wn_index;
+    uint32_t* level;         // level l = slots [level[l], level[l + 1])
+};
+
+__device__ __forceinline__ bool wb_encloses(const hk_node& o, const hk_node& in) {
+    bool r = true;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) r = r && o.min[k] <= in.min[k] && in.max[k] <= o.max[k];       // false for NaN, as the host
+    return r;
+}
+
+// Parser::range over [p, end): the branches' records, their count | WB_OK when every link nests and `box` (if any) encloses them
+__device__ uint32_t wb_branches(const hk_node* flat, uint32_t p, uint32_t end, const hk_node* box, uint4& kids) {
+    uint32_t k = 0u, at[4] = {0u, 0u, 0u, 0u};
+    bool ok = p < end;
+    while (ok && p < end) {
+        if (k == 4u) { ok = false; break; }
+        const hk_node q = flat[p];
+        if (q.entry_index != p + 1u || q.exit_index <= p + 1u || q.exit_index > end) { ok = false; break; }
+        if (box && !wb_encloses(*box, q)) ok = false;
+        at[k++] = p;
+        p = q.exit_index;
+    }
+    kids = make_uint4(at[0], at[1], at[2], at[3]);
+    return k | (ok ? WB_OK : 0u);
+}
+
+__device__ __forceinline__ float wb_half_area(const hk_node& b) {
+    const float sx = smax(b.max[0] - b.min[0], 0.0f), sy = smax(b.max[1] - b.min[1], 0.0f), sz = smax(b.max[2] - b.min[2], 0.0f);
+    return sx * sy + sx * sz + sy * sz;
+}
+
+// a branch found at range depth `depth`: its own parse succeeded, and a navigator with branches stays within the recursion limit
+__device__ __forceinline__ bool wb_branch_ok(uint32_t meta, uint32_t depth) {
+    return (meta & WB_OK) != 0u && ((meta & WB_LEAF) != 0u || depth + 1u <= WB_MAX_DEPTH);
+}
+
+__global__ void __launch_bounds__(256) kc_build_wide_tlas(uint32_t n, const hk_node* __restrict__ flat, uint32_t blas_ok, uint32_t base_need,
+                                                          WideScratch s, hk_wide_node* nodes, uint32_t* rank, uint32_t* state) {
+    __shared__ uint32_t s_scan[256];
+    __shared__ uint32_t s_total;
+    const uint32_t tid = threadIdx.x, threads = blockDim.x;
+    if (n == 0u) return;
+    if (n == 1u) {          // one leaf record without a navigator: root = WIDE_LEAF | 0, no nodes
+        if (tid == 0u) {
+            const uint32_t e = flat[0].entry_index;
+            const bool ok = e >= SCENE_LEAF && e - SCENE_LEAF < n;
+            rank[0] = 0u;
+            state[0] = (blas_ok && ok && base_need <= (uint32_t)HK_WIDE_STACK) ? 1u : 0u;
+            state[1] = base_need; state[2] = 0u;
+        }
+        return;
+    }
+    const uint32_t count = 3u * n - 2u, cap = n - 1u;       // a binary tree over n shapes collapses into at most n - 1 wide nodes
+    bool bad = false;
+    // ---- parse: every record as a navigator, and the top-level range
+    for (uint32_t i = tid; i <= count; i += threads) {
+        uint32_t meta = 0u;
+        uint4 kids = make_uint4(0u, 0u, 0u, 0u);
+        if (i == count) {
+            meta = wb_branches(flat, 0u, count, nullptr, kids);
+        } else {
+            const hk_node nav = flat[i];
+            if (nav.entry_index < SCENE_LEAF && i + 1u < count) {
+                const hk_node first = flat[i + 1u];
+                if (first.entry_index >= SCENE_LEAF) {
+                    const uint32_t shape = first.entry_index - SCENE_LEAF;
+                    kids.x = shape;
+                    meta = WB_LEAF | ((nav.exit_index == i + 2u && first.exit_index == i + 2u && shape < n) ? WB_OK : 0u);
+                } else if (nav.exit_index <= count) {
+                    meta = wb_branches(flat, i + 1u, nav.exit_index, &nav, kids);
+                }
+            }
+        }
+        s.rec_meta[i] = meta;
+        s.rec_kids[i] = kids;
+    }
+    // ---- ranks: leaf records before each leaf record, in per-thread chunks of the array
+    for (uint32_t i = tid; i < n; i += threads) rank[i] = 0xFFFFFFFFu;
+    const uint32_t chunk = (count + threads - 1u) / threads, c0 = min(count, tid * chunk), c1 = min(count, c0 + chunk);
+    uint32_t leaves = 0u;
+    for (uint32_t i = c0; i < c1; ++i) leaves += flat[i].entry_index >= SCENE_LEAF ? 1u : 0u;
+    s_scan[tid] = leaves;
+    if (tid == 0u) {
+        s.wn_bin[0] = count; s.wn_depth[0] = 0u; s.wn_index[0] = 0u;
+        s.level[0] = 0u; s.level[1] = 1u;
+        s_total = 1u;
+    }
+    __syncthreads();
+    for (uint32_t o = 1u; o < threads; o <<= 1) {
+        const uint32_t v = tid >= o ? s_scan[tid - o] : 0u;
+        __syncthreads();
+        s_scan[tid] += v;
+        __syncthreads();
+    }
+    const uint32_t first_rank = s_scan[tid] - leaves;
+    uint32_t r = first_rank;
+    for (uint32_t i = c0; i < c1; ++i) {
+        const uint32_t e = flat[i].entry_index;
+        if (e < SCENE_LEAF) continue;
+        if (e - SCENE_LEAF < n) rank[e - SCENE_LEAF] = r;
+        ++r;
+    }
+    __syncthreads();
+    r = first_rank;
+    for (uint32_t i = c0; i < c1; ++i) {       // a shape named twice keeps only one of its ranks
+        const uint32_t e = flat[i].entry_index;
+        if (e < SCENE_LEAF) continue;
+        if (e - SCENE_LEAF < n && rank[e - SCENE_LEAF] != r) bad = true;
+        ++r;
+    }
+    // ---- collapse, level by level
+    {
+        const uint32_t m = s.rec_meta[count];
+        if (!wb_branch_ok(m, 0u) || (m & WB_LEAF) != 0u) bad = true;
+    }
+    uint32_t lb = 0u, le = 1u, levels = 0u;
+    while (lb < le) {
+        for (uint32_t w = lb + tid; w < le; w += threads) {
+            const uint32_t b = s.wn_bin[w], depth = s.wn_depth[w], meta = s.rec_meta[b];
+            bool ok = (meta & WB_OK) != 0u && (meta & WB_LEAF) == 0u;
+            uint32_t k = ok ? (meta & 7u) : 0u, id[4], dp[4];
+            const uint4 bk = s.rec_kids[b];
+            id[0] = bk.x; id[1] = bk.y; id[2] = bk.z; id[3] = bk.w;
+            for (uint32_t j = 0u; j < 4u; ++j) dp[j] = depth;
+            for (uint32_t j = 0u; j < k; ++j) ok = ok && wb_branch_ok(s.rec_meta[id[j]], dp[j]);
+            while (ok && k < 4u) {
+                int open = -1;
+                float best = -1.0f;
+                for (uint32_t j = 0u; j < k; ++j) {
+                    const uint32_t mj = s.rec_meta[id[j]];
+                    if ((mj & WB_LEAF) != 0u || k - 1u + (mj & 7u) > 4u) continue;
+                    const float a = wb_half_area(flat[id[j]]);
+                    if (a > best) { best = a; open = (int)j; }
+                }
+                if (open < 0) break;
+                const uint32_t o = (uint32_t)open, mo = s.rec_meta[id[o]], sk = mo & 7u, sd = dp[o] + 1u;
+                const uint4 sub4 = s.rec_kids[id[o]];
+                const uint32_t sub[4] = {sub4.x, sub4.y, sub4.z, sub4.w};
+                for (uint32_t j = k; j-- > o + 1u;) { id[j + sk - 1u] = id[j]; dp[j + sk - 1u] = dp[j]; }    // the rest moves up by sk - 1
+                for (uint32_t j = 0u; j < sk; ++j) {
+                    id[o + j] = sub[j]; dp[o + j] = sd;
+                    ok = ok && wb_branch_ok(s.rec_meta[sub[j]], sd);
+                }
+                k += sk - 1u;
+            }
+            uint32_t child[4] = {WIDE_EMPTY, WIDE_EMPTY, WIDE_EMPTY, WIDE_EMPTY};
+            if (!ok) k = 0u;
+            for (uint32_t c = 0u; c < k; ++c) {
+                if ((s.rec_meta[id[c]] & WB_LEAF) != 0u) continue;
+                const uint32_t slot = atomicAdd(&s_total, 1u);
+                if (slot >= cap) { ok = false; continue; }
+                s.wn_bin[slot] = id[c]; s.wn_depth[slot] = dp[c] + 1u;
+                child[c] = slot;
+            }
+            bad = bad || !ok;
+            s.wn_k[w] = k;
+            s.wn_kids[w] = make_uint4(id[0], id[1], id[2], id[3]);
+            s.wn_child[w] = make_uint4(child[0], child[1], child[2], child[3]);
+        }
+        __syncthreads();
+        lb = le;
+        le = min(*(volatile uint32_t*)&s_total, cap);
+        ++levels;
+        if (tid == 0u) s.level[levels + 1u] = le;
+        __syncthreads();
+    }
+    const bool ok = __syncthreads_or(bad ? 1 : 0) == 0;
+    if (ok) {
+        // ---- sizes and needs, bottom-up
+        for (uint32_t l = levels; l-- > 0u;) {
+            const uint32_t l0 = s.level[l], l1 = s.level[l + 1u];
+            for (uint32_t w = l0 + tid; w < l1; w += threads) {
+                const uint32_t k = s.wn_k[w];
+                const uint4 c4 = s.wn_child[w];
+                const uint32_t ch[4] = {c4.x, c4.y, c4.z, c4.w};
+                uint32_t size = 1u, need = 0u;
+                for (uint32_t c = 0u; c < k; ++c) {
+                    uint32_t sub = 0u;
+                    if (ch[c] != WIDE_EMPTY) { size += s.wn_size[ch[c]]; sub = s.wn_need[ch[c]]; }
+                    need = max(need, (k - 1u) + sub);
+                }
+                s.wn_size[w] = size; s.wn_need[w] = need;
+            }
+            __syncthreads();
+        }
+        // ---- pre-order indices and nodes, top-down
+        const float inf = __uint_as_float(0x7f800000u), ninf = __uint_as_float(0xff800000u);
+        for (uint32_t l = 0u; l < levels; ++l) {
+            const uint32_t l0 = s.level[l], l1 = s.level[l + 1u];
+            for (uint32_t w = l0 + tid; w < l1; w += threads) {
+                const uint32_t k = s.wn_k[w], index = s.wn_index[w];
+                const uint4 k4 = s.wn_kids[w], c4 = s.wn_child[w];
+                const uint32_t id[4] = {k4.x, k4.y, k4.z, k4.w}, ch[4] = {c4.x, c4.y, c4.z, c4.w};
+                float v[6][4];
+                uint32_t ref[4];
+                uint32_t next = index + 1u;
+                for (uint32_t c = 0u; c < 4u; ++c) {
+                    if (c >= k) {
+                        v[0][c] = v[1][c] = v[2][c] = inf; v[3][c] = v[4][c] = v[5][c] = ninf;
+                        ref[c] = WIDE_EMPTY;
+                        continue;
+                    }
+                    const hk_node b = flat[id[c]];
+                    v[0][c] = b.min[0]; v[1][c] = b.min[1]; v[2][c] = b.min[2];
+                    v[3][c] = b.max[0]; v[4][c] = b.max[1]; v[5][c] = b.max[2];
+                    if (ch[c] != WIDE_EMPTY) {
+                        s.wn_index[ch[c]] = next;
+                        ref[c] = next;
+                        next += s.wn_size[ch[c]];
+                    } else {
+                        ref[c] = WIDE_LEAF | s.rec_kids[id[c]].x;
+                    }
+                }
+                float4* out = reinterpret_cast<float4*>(nodes + index);
+                for (int q = 0; q < 6; ++q) out[q] = make_float4(v[q][0], v[q][1], v[q][2], v[q][3]);
+                reinterpret_cast<uint4*>(out)[6] = make_uint4(ref[0], ref[1], ref[2], ref[3]);
+                reinterpret_cast<uint4*>(out)[7] = make_uint4(0u, 0u, 0u, 0u);
+            }
+            __syncthreads();
+        }
+    } else {
+        for (uint32_t i = tid; i < n; i += threads) rank[i] = 0u;
+    }
+    if (tid == 0u) {
+        const uint32_t need = (ok ? s.wn_need[0] : 0u) + base_need;
+        state[0] = (blas_ok && ok && need <= (uint32_t)HK_WIDE_STACK) ? 1u : 0u;
+        state[1] = need;
+        state[2] = ok ? s.wn_size[0] : 0u;
+    }
+}
+
 }  // namespace hkd
 
 // ------------------------------------------------------------------------------------------------ launchers
@@ -447,6 +709,34 @@ void hk_launch_build_flat_bvh(uint32_t n, const float4* box_lo, const float4* bo
 }
 size_t hk_scene_bvh_scratch_bytes(uint32_t n) {
     return sizeof(float4) * (size_t)n + 2u * sizeof(uint32_t) * (size_t)n + 16u + 2u * sizeof(hkd::BuildSeg) * (size_t)n;
+}
+// scratch: rec_kids uint4[3n - 1] | wn_kids, wn_child uint4[n - 1] | rec_meta uint32[3n - 1] | six uint32[n - 1] | level uint32[n + 1]
+static hkd::WideScratch wide_scratch(uint32_t n, void* scratch) {
+    const size_t recs = n < 2u ? 2u : 3u * (size_t)n - 1u, cap = n < 2u ? 1u : (size_t)n - 1u;
+    hkd::WideScratch s;
+    uint4* q = reinterpret_cast<uint4*>(scratch);
+    s.rec_kids = q; q += recs;
+    s.wn_kids = q; q += cap;
+    s.wn_child = q; q += cap;
+    uint32_t* u = reinterpret_cast<uint32_t*>(q);
+    s.rec_meta = u; u += recs;
+    s.wn_bin = u; u += cap;
+    s.wn_depth = u; u += cap;
+    s.wn_k = u; u += cap;
+    s.wn_size = u; u += cap;
+    s.wn_need = u; u += cap;
+    s.wn_index = u; u += cap;
+    s.level = u;
+    return s;
+}
+size_t hk_wide_tlas_scratch_bytes(uint32_t n) {
+    const size_t recs = n < 2u ? 2u : 3u * (size_t)n - 1u, cap = n < 2u ? 1u : (size_t)n - 1u;
+    return 16u * (recs + 2u * cap) + 4u * (recs + 6u * cap + cap + 2u);
+}
+void hk_launch_build_wide_tlas(uint32_t n, const hk_node* flat, bool blas_ok, uint32_t base_need, void* scratch, hkd::hk_wide_node* nodes,
+                               uint32_t* rank, uint32_t* state, cudaStream_t st) {
+    if (n == 0u) return;
+    kc_build_wide_tlas<<<1, 256, 0, st>>>(n, flat, blas_ok ? 1u : 0u, base_need, wide_scratch(n, scratch), nodes, rank, state);
 }
 void hk_launch_scene_emissives(uint32_t ne, hk_emissive* emissives, const hk_instance* instances, const hk_material* materials,
                                const hk_primitive* primitives, const hk_vertex* vertices, float4* box_lo, float4* box_hi, cudaStream_t st) {

@@ -119,6 +119,10 @@ OUT_GBUFFER_POSITION, OUT_GBUFFER_NORMAL, OUT_GBUFFER_DEPTH_GRADIENT = 16, 17, 1
 OUT_GBUFFER_INSTANCE_MATERIAL, OUT_GBUFFER_VELOCITY_UV = 19, 20
 OUT_RESERVOIR_0 = 32
 SCENE_INSTANCES, SCENE_INSTANCE_NODES, SCENE_EMISSIVES, SCENE_EMISSIVE_NODES, SCENE_PREVIOUS_MODELS, SCENE_INSTANCE_MOVED = range(6)   # hk_scene_readback
+SCENE_WIDE_TLAS, SCENE_WIDE_INSTANCE_RANK = 6, 7
+WIDE_NODE = np.dtype([("lo_x", f4, 4), ("lo_y", f4, 4), ("lo_z", f4, 4), ("hi_x", f4, 4), ("hi_y", f4, 4), ("hi_z", f4, 4),
+                      ("child", u4, 4), ("pad", u4, 4)])      # hk_wide_node (csrc/hk_wide.cuh), 128 bytes
+assert WIDE_NODE.itemsize == 128
 
 # bytes per pixel and numpy view of each read-back plane
 OUT_FORMATS = {}

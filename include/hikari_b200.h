@@ -197,8 +197,10 @@ int hk_scene_update_instances(hk_context* ctx, const hk_scene_desc* scene);
  * and the alias tables, which the reference rebuilds when an emissive instance's scale moved by more than 0.01 (instance.rs:385-397;
  * hikari::MeshMaterialWorld::prepare_instance_transforms checks both and says when hk_scene_update_instances is needed instead).
  * HK_ERR_UNSUPPORTED if the uploaded TLAS / emissive BVH is not in bvh 0.7.1's layout.  When rays walk the 4-wide trees
- * (HK_TUNE_WIDE_TRAVERSAL in effect for this scene) the 4-wide TLAS is re-derived on the host from the records just built, which
- * costs one small read-back and a stream synchronisation; otherwise the call never waits for the device. */
+ * (HK_TUNE_WIDE_TRAVERSAL in effect for this scene) one more kernel derives the 4-wide TLAS on the device from the records just built,
+ * node for node what hk_scene_upload derives on the host, and decides there whether it fits the walk's stack: a frame whose TLAS does
+ * not fit walks the reference's arrays for every ray, and hk_get_stats (which then waits for the scene's stream) reports it.  The
+ * call never waits for the device, except for its pinned staging slot when the host is two calls ahead of the copies. */
 int hk_scene_update_transforms(hk_context* ctx, const float* models, const float* previous_models, const float* mesh_aabbs,
                                uint32_t instance_count);
 /* Shared scenes: several cameras render ONE scene, uploaded and animated once per frame.  The reference keeps one set of scene
@@ -222,10 +224,9 @@ int hk_scene_update_transforms(hk_context* ctx, const float* models, const float
  *     the last launch of its last frame call that reads the scene (hk_prepass_run, hk_light_run, hk_run_pass, hk_trace_rays,
  *     hk_render_frame), then rewrites the buffers; such a context's next frame waits for the update on the device.  No buffer a
  *     camera may still read is freed before that camera has finished with it.  Nothing is waited for on the host except where the
- *     hk_scene_* calls already synchronise (full uploads, instance updates, the 4-wide TLAS read-back of hk_scene_update_transforms,
- *     which with a shared scene also waits for the cameras' frames in flight).  A context on the scene's own stream records and
- *     waits for nothing: stream order already holds.
- *   - hk_shared_scene_update_transforms re-derives the 4-wide TLAS when ANY attached context walks the 4-wide trees
+ *     hk_scene_* calls already synchronise (full uploads, instance updates); hk_shared_scene_update_transforms does not wait for
+ *     the cameras' frames in flight.  A context on the scene's own stream records and waits for nothing: stream order already holds.
+ *   - hk_shared_scene_update_transforms re-derives the 4-wide TLAS on the device when ANY attached context walks the 4-wide trees
  *     (HK_TUNE_WIDE_TRAVERSAL stays a per-context setting).
  *   - Threading: a scene and every context attached to it are driven from one thread at a time (Bevy 0.9's render graph does this).
  * Errors of the hk_shared_scene_* calls are reported by hk_shared_scene_last_error(s) (s = NULL: the last failed create). */
@@ -240,7 +241,9 @@ const char* hk_shared_scene_last_error(hk_shared_scene* s);
 int hk_context_attach_scene(hk_context* ctx, hk_shared_scene* s);   /* NULL detaches; frees a private scene */
 /* Test / debugging aid: the per-frame scene buffers as they are on the device, in the layouts of hk_layout.h. */
 enum { HK_SCENE_INSTANCES = 0, HK_SCENE_INSTANCE_NODES = 1, HK_SCENE_EMISSIVES = 2, HK_SCENE_EMISSIVE_NODES = 3,
-       HK_SCENE_PREVIOUS_MODELS = 4 /* 64 B per instance; empty when nothing moved */, HK_SCENE_INSTANCE_MOVED = 5 /* uint32 per instance */ };
+       HK_SCENE_PREVIOUS_MODELS = 4 /* 64 B per instance; empty when nothing moved */, HK_SCENE_INSTANCE_MOVED = 5 /* uint32 per instance */,
+       HK_SCENE_WIDE_TLAS = 6 /* the 4-wide TLAS of HK_TUNE_WIDE_TRAVERSAL: 128-B nodes (csrc/hk_wide.cuh); empty when it could not be derived */,
+       HK_SCENE_WIDE_INSTANCE_RANK = 7 /* uint32 per instance: its leaf's position among the TLAS's leaf records */ };
 int hk_scene_buffer_bytes(hk_context* ctx, int which, size_t* bytes);
 int hk_scene_readback(hk_context* ctx, int which, void* host, size_t bytes);   /* bytes = hk_scene_buffer_bytes */
 int hk_set_noise(hk_context* ctx, const uint8_t* rgba8_64x64x16);   /* 16 textures of 64x64 RGBA8, lib.rs:189-219 */
@@ -354,7 +357,9 @@ int hk_set_profiling_kernel(hk_context* ctx, int kernel);
  * when one of its flat arrays is not in that layout, names a shape in two leaves, has a run of more than four branches below a
  * navigator or at the top level, or has a navigator box that does not enclose the boxes below it (its children's navigators, or
  * the shape's own box at a leaf), or when its trees could overflow the walk's stack (hk_frame_stats.wide_traversal: bit 0 =
- * primary rays, bit 1 = light passes). */
+ * primary rays, bit 1 = light passes).  After hk_scene_update_transforms the 4-wide TLAS is derived on the device (see there): the
+ * stack check is made per update, on the device, and mode 1's 256-node rule counts the 4-wide TLAS of the last hk_scene_upload /
+ * hk_scene_update_instances (the host does not learn the node count of a tree derived on the device). */
 enum { HK_TUNE_POOLED_INDIRECT = 1, HK_TUNE_TILED_SPATIAL = 2, HK_TUNE_TILED_DENOISE = 3, HK_TUNE_WIDE_TRAVERSAL = 4 };
 int hk_set_tuning(hk_context* ctx, int key, int value);
 int hk_set_keep_intermediates(hk_context* ctx, int keep);   /* 1: hk_render_frame also writes HK_OUT_DENOISED_* */

@@ -97,8 +97,7 @@ def run_arm(spec, shared, one_stream, frames, warmup):
     torch.cuda.synchronize()
     frame_s = (time.perf_counter() - t_run) / frames
     # the update(s) alone with the device idle before each call: the host's own work, without the back-pressure of the frames in
-    # flight that the frame time above contains (pinned staging slots, and the 4-wide TLAS read-back when a camera walks the 4-wide
-    # trees, which waits for the scene's stream)
+    # flight that the frame time above contains (the pinned staging slot of two calls before)
     for f in range(warmup + frames + 1, warmup + frames + 9):
         for k, track in an.tracks.items():
             world.set_instance_transform(k, an.compose(track(f), an.base[k]))
