@@ -830,10 +830,33 @@ static int upload_instances(hk_shared_scene* sc, const hk_scene_desc* s, DeviceS
     return upload_wide(sc, s, d);
 }
 
+// A model matrix with an infinite or NaN entry has no world box and no place in the TLAS (the SAH build's bucket of a NaN centre is
+// undefined, and differently so on the host and the device): refused on the host, before anything is built, launched or freed, so
+// that the scene stays as it was.  Singular but finite models (an axis scaled to zero) are accepted, as the reference accepts them.
+static int check_models(hk_shared_scene* sc, const float* models, size_t stride_floats, uint32_t n, const char* what) {
+    for (uint32_t i = 0; i < n; ++i) {
+        const float* m = models + stride_floats * (size_t)i;
+        for (int k = 0; k < 16; ++k) {
+            uint32_t bits;
+            memcpy(&bits, m + k, 4);
+            if ((bits & 0x7f800000u) == 0x7f800000u)
+                return set_error(sc, HK_ERR_INVALID_ARGUMENT, std::string(what) + ": instance " + std::to_string(i) + " has a non-finite model matrix (entry " +
+                                                              std::to_string(k) + ")");
+        }
+    }
+    return HK_OK;
+}
+static int check_instance_models(hk_shared_scene* sc, const hk_scene_desc* s, const char* what) {
+    if (!s->instance_count || !s->instances) return HK_OK;     // (a NULL pointer is reported by upload_instances)
+    static_assert(sizeof(hk_instance) % sizeof(float) == 0, "instance records are float-aligned");
+    return check_models(sc, s->instances[0].model, sizeof(hk_instance) / sizeof(float), s->instance_count, what);
+}
+
 static int scene_upload(hk_shared_scene* sc, const hk_scene_desc* s) {
     if ((s->vertex_count && !s->vertices) || (s->primitive_count && !s->primitives) ||
         (s->material_count && !s->materials) || (s->asset_node_count && !s->asset_nodes) || (s->texture_count && !s->textures))
         return set_error(sc, HK_ERR_INVALID_ARGUMENT, "scene buffer pointer is NULL with a non-zero count");
+    if (const int rc = check_instance_models(sc, s, "hk_scene_upload")) return rc;
     bool boxes_match = true;
     auto same3 = [](const float* a, const float* b) { return a[0] == b[0] && a[1] == b[1] && a[2] == b[2]; };
     std::unordered_set<uint32_t> checked;   // mesh node ranges repeat across instances: check each once
@@ -929,6 +952,7 @@ static int scene_upload(hk_shared_scene* sc, const hk_scene_desc* s) {
 
 static int scene_update_instances(hk_shared_scene* sc, const hk_scene_desc* s) {
     if (!sc->ready) return set_error(sc, HK_ERR_NOT_READY, "hk_scene_update_instances needs a scene from hk_scene_upload");
+    if (const int rc = check_instance_models(sc, s, "hk_scene_update_instances")) return rc;
     HK_SCUDA(cudaSetDevice(sc->device));
     DeviceScene d = sc->scene;
     int rc = upload_instances(sc, s, d);
@@ -954,6 +978,15 @@ static int scene_update_transforms(hk_shared_scene* sc, const float* models, con
                                                        "(a changed set goes through hk_scene_update_instances)");
     const uint32_t n = instance_count, ne = sc->scene_emissive_count;
     if (n == 0u) return HK_OK;
+    if (const int rc = check_models(sc, models, 16, n, "hk_scene_update_transforms")) return rc;
+    for (uint32_t i = 0; i < n; ++i)          // a non-finite mesh AABB gives a non-finite centre just as a model does
+        for (int k = 0; k < 6; ++k) {
+            uint32_t bits;
+            memcpy(&bits, mesh_aabbs + 6 * (size_t)i + k, 4);
+            if ((bits & 0x7f800000u) == 0x7f800000u)
+                return set_error(sc, HK_ERR_INVALID_ARGUMENT, "hk_scene_update_transforms: instance " + std::to_string(i) +
+                                                              " has a non-finite mesh AABB (entry " + std::to_string(k) + ")");
+        }
     DeviceScene d = sc->scene;
     // the arrays being rebuilt in place must have bvh 0.7.1's sizes (3 m - 2 records over m >= 2 shapes, 1 over one)
     const uint32_t tlas_records = n == 1u ? 1u : 3u * n - 2u, em_records = ne == 0u ? 0u : (ne == 1u ? 1u : 3u * ne - 2u);

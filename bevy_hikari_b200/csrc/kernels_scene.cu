@@ -136,10 +136,16 @@ __device__ void mat4_inverse_dev(const float* m, float* out) {
     const float d0 = m00 * inv[0][0], d1 = m01 * inv[1][0], d2 = m02 * inv[2][0], d3 = m03 * inv[3][0];
     const float dot1 = ((d0 + d1) + d2) + d3;
     const float rcp_det = 1.0f / dot1;
+    // A singular model (an axis scaled to zero) gives rcp_det = ±inf and 0 * inf = NaN in every zero cofactor.  The device writes
+    // every NaN as 0x7FFFFFFF; x86 writes its default NaN 0xFFC00000, and with finite inputs every NaN of this expansion is that one
+    // (generated, then only propagated).  The reference uploads the x86 bytes, and so does the host path: write those.
 #pragma unroll
     for (int c = 0; c < 4; ++c)
 #pragma unroll
-        for (int k = 0; k < 4; ++k) out[4 * c + k] = inv[c][k] * rcp_det;
+        for (int k = 0; k < 4; ++k) {
+            const float v = inv[c][k] * rcp_det;
+            out[4 * c + k] = v != v ? __uint_as_float(0xFFC00000u) : v;
+        }
 }
 
 }  // namespace

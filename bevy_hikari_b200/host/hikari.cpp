@@ -66,6 +66,13 @@ constexpr float BVH_EPSILON = 0.00001f;
 constexpr int NUM_BUCKETS = 6;
 const float INF = std::numeric_limits<float>::infinity();
 
+// Rust's `f32 as usize`: saturating, NaN -> 0 (a C++ cast of NaN or of a negative value is undefined)
+size_t rust_as_usize(float x) {
+    if (!(x > 0.0f)) return 0;
+    if (x >= 18446744073709551616.0f) return std::numeric_limits<size_t>::max();
+    return (size_t)x;
+}
+
 struct Box {
     float mn[3] = {INF, INF, INF};
     float mx[3] = {-INF, -INF, -INF};
@@ -137,7 +144,8 @@ struct Builder {
             std::vector<uint32_t> assign[NUM_BUCKETS];
             for (uint32_t i : indices) {
                 float rel = (centers[i][axis] - centroid_bounds.mn[axis]) / split_axis_size;
-                size_t bucket = (size_t)(rel * ((float)NUM_BUCKETS - 0.01f));
+                size_t bucket = rust_as_usize(rel * ((float)NUM_BUCKETS - 0.01f));
+                if (bucket >= (size_t)NUM_BUCKETS) bucket = NUM_BUCKETS - 1;    // only for non-finite boxes (bvh 0.7.1 panics there)
                 b_size[bucket] += 1;
                 b_box[bucket].join(boxes[i]);
                 assign[bucket].push_back(i);
@@ -153,6 +161,16 @@ struct Builder {
             }
             for (int b = 0; b <= min_bucket; ++b) l_idx.insert(l_idx.end(), assign[b].begin(), assign[b].end());
             for (int b = min_bucket + 1; b < NUM_BUCKETS; ++b) r_idx.insert(r_idx.end(), assign[b].begin(), assign[b].end());
+            if (l_idx.empty() || r_idx.empty()) {
+                // Finite boxes put the smallest centre in bucket 0 and the largest in bucket 5, so both sides hold a shape.  Only
+                // non-finite boxes (NaN centres, NaN costs) get here; the halves keep the build finite.  The library refuses such
+                // a scene at upload (hk_scene_upload), but this builder runs first.
+                const size_t half = indices.size() / 2;
+                l_idx.assign(indices.begin(), indices.begin() + half);
+                r_idx.assign(indices.begin() + half, indices.end());
+                l_box = joint(l_idx, 0, l_idx.size());
+                r_box = joint(r_idx, 0, r_idx.size());
+            }
         }
         uint32_t l = build(l_idx);
         uint32_t r = build(r_idx);
@@ -264,6 +282,22 @@ void mat4_inverse(const float m[16], float out[16]) {
         for (int k = 0; k < 4; ++k) out[4 * c + k] = inv[c][k] * rcp_det;
 }
 float length3(const float a[3]) { return sqrtf((a[0] * a[0] + a[1] * a[1]) + a[2] * a[2]); }
+
+// The alias-table cache rule of instance.rs:385-397, used both where prepare_instances decides whether to rebuild a light's table
+// and where prepare_instance_transforms decides whether an update may stay on the device.
+// glam Mat4::to_scale_rotation_translation().0 = (|x_axis| * det.signum(), |y_axis|, |z_axis|), with Rust's f32::signum: -1 for
+// negative values and -0.0, +1 for positive values and +0.0, NaN for NaN.  det = the upper 3x3's, as the model is affine.
+void scale_of(const float* m, float scale[3]) {
+    const float det3 = m[0] * (m[5] * m[10] - m[6] * m[9]) - m[4] * (m[1] * m[10] - m[2] * m[9]) + m[8] * (m[1] * m[6] - m[2] * m[5]);
+    const float signum = det3 != det3 ? det3 : copysignf(1.0f, det3);
+    scale[0] = length3(m) * signum;
+    scale[1] = length3(m + 4);
+    scale[2] = length3(m + 8);
+}
+// Vec3::abs_diff_eq(other, 0.01): every |a - b| <= 0.01, so false when any component is NaN
+bool scale_within(const float a[3], const float b[3]) {
+    return fabsf(a[0] - b[0]) <= 0.01f && fabsf(a[1] - b[1]) <= 0.01f && fabsf(a[2] - b[2]) <= 0.01f;
+}
 
 }  // namespace
 
@@ -488,16 +522,9 @@ void MeshMaterialWorld::prepare_instances() {  // instance.rs:245-444
             // alias table cached per entity while the scale stays within 0.01 (instance.rs:385-397): a rotating or
             // translating light keeps the table computed for the transform it was first seen with
             float scale[3];
-            {   // glam Mat4::to_scale_rotation_translation().0 = (|x_axis| * signum(det), |y_axis|, |z_axis|)
-                const float* m = inst.model;
-                float det3 = m[0] * (m[5] * m[10] - m[6] * m[9]) - m[4] * (m[1] * m[10] - m[2] * m[9]) + m[8] * (m[1] * m[6] - m[2] * m[5]);
-                scale[0] = length3(m) * (det3 < 0.0f ? -1.0f : 1.0f);
-                scale[1] = length3(m + 4);
-                scale[2] = length3(m + 8);
-            }
+            scale_of(inst.model, scale);
             CachedAliasTable& cache = alias_table_cache_[(size_t)(kept[id] - instances_in_.data())];
-            const bool cache_hit = cache.valid && fabsf(cache.scale[0] - scale[0]) <= 0.01f && fabsf(cache.scale[1] - scale[1]) <= 0.01f &&
-                                   fabsf(cache.scale[2] - scale[2]) <= 0.01f;
+            const bool cache_hit = cache.valid && scale_within(cache.scale, scale);
             if (!cache_hit) {
                 cache.valid = true;
                 memcpy(cache.scale, scale, 12);
@@ -530,13 +557,6 @@ void MeshMaterialWorld::prepare_instances() {  // instance.rs:245-444
     }
 }
 
-static void scale_of(const float* m, float scale[3]) {   // glam Mat4::to_scale_rotation_translation().0
-    float det3 = m[0] * (m[5] * m[10] - m[6] * m[9]) - m[4] * (m[1] * m[10] - m[2] * m[9]) + m[8] * (m[1] * m[6] - m[2] * m[5]);
-    scale[0] = length3(m) * (det3 < 0.0f ? -1.0f : 1.0f);
-    scale[1] = length3(m + 4);
-    scale[2] = length3(m + 8);
-}
-
 bool MeshMaterialWorld::prepare_instance_transforms() {
     if (!universal_settings.build_instance_acceleration_structure) return false;
     std::vector<const InstanceDesc*> kept;
@@ -556,8 +576,7 @@ bool MeshMaterialWorld::prepare_instance_transforms() {
         if (entity >= alias_table_cache_.size() || !alias_table_cache_[entity].valid) return false;
         float scale[3];
         scale_of(d->transform, scale);
-        const CachedAliasTable& c = alias_table_cache_[entity];
-        if (!(fabsf(c.scale[0] - scale[0]) <= 0.01f && fabsf(c.scale[1] - scale[1]) <= 0.01f && fabsf(c.scale[2] - scale[2]) <= 0.01f)) return false;
+        if (!scale_within(alias_table_cache_[entity].scale, scale)) return false;
     }
     mesh_aabb_.resize(meshes_.size());
     mesh_aabb_ok_.resize(meshes_.size(), false);

@@ -175,6 +175,15 @@ int hk_context_resize_tile(hk_context* ctx, uint32_t width, uint32_t height, uin
                            uint32_t row_begin, uint32_t row_end);
 int hk_reset_temporal_state(hk_context* ctx);   /* zero reservoirs, as re-allocation does in light.rs:342-363 */
 
+/* Model matrices must be finite.  hk_scene_upload, hk_scene_update_instances (instances[i].model), hk_scene_update_transforms
+ * (models) and their hk_shared_scene_* forms check all 16 floats of every instance on the host before anything is built, launched
+ * or freed, and return HK_ERR_INVALID_ARGUMENT for an infinite or NaN entry; hk_last_error names the call, the instance and the
+ * entry; hk_scene_update_transforms checks its mesh_aabbs the same way.  The scene stays as it was, and the next valid call works.
+ * previous_models are not checked: they only enter the motion vectors, and the frame after a refused update legitimately hands
+ * the refused matrix back as the previous one (GlobalTransformQueue[1]); a non-finite entry gives that instance NaN velocities for
+ * one frame and builds nothing.  Singular but finite models (an axis scaled to zero, a Bevy
+ * spawn or hide animation) are accepted, as in the reference: their inverse-transpose matrix holds NaNs, written as x86's default
+ * NaN 0xFFC00000 by both the host and the device path, and rays miss them. */
 int hk_scene_upload(hk_context* ctx, const hk_scene_desc* scene);
 /* The per-frame part of the scene, for animated instances and materials: replaces instances, instance_nodes (TLAS), emissives,
  * emissive_nodes, alias_table and previous_instance_models — what MeshMaterialRenderAssets / InstanceRenderAssets::set +

@@ -198,7 +198,9 @@ pub fn upload_scene(scene: &HikariB200Scene, desc: &ffi::hk_scene_desc, instance
 /// `models` / `previous_models`: `GlobalTransform::compute_matrix().to_cols_array()` of every instance in instance order and its
 /// `GlobalTransformQueue[1]`; `mesh_aabbs`: `[center.x, center.y, center.z, half.x, half.y, half.z]` of each instance's mesh `Aabb`.
 /// The caller keeps the reference's conditions for the full path (instance set changed, or an emissive's scale left its cached alias
-/// table's +-0.01 range, instance.rs:385-397) and calls `upload_scene(.., instances_only = true)` then.
+/// table's +-0.01 range, instance.rs:385-397) and calls `upload_scene(.., instances_only = true)` then.  A model with an infinite
+/// or NaN entry is refused here and by `upload_scene` (`HK_ERR_INVALID_ARGUMENT`, logged with the instance it names): the scene
+/// stays as it was.
 pub fn update_transforms(scene: &HikariB200Scene, models: &[[f32; 16]], previous_models: Option<&[[f32; 16]]>, mesh_aabbs: &[[f32; 6]]) -> bool {
     debug_assert!(models.len() == mesh_aabbs.len() && previous_models.map_or(true, |p| p.len() == models.len()));
     let rc = unsafe {

@@ -10,6 +10,8 @@ echo "== generated Rust declarations current";                           python 
 echo "== AddressSanitizer build of the emulated kernels on the newest device tests"
 LD_PRELOAD=$(g++ -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 HK_EMULATE_KERNELS=1 HK_EMU_ASAN=1 \
     python -m pytest tests/test_gpu_zz_fsr.py tests/test_gpu_zz_examples.py tests/test_gpu_upscale.py -m gpu -q -x -p no:cacheprovider
+LD_PRELOAD=$(g++ -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 HK_EMULATE_KERNELS=1 HK_EMU_ASAN=1 \
+    python -m pytest tests/test_gpu_scene_update_edges.py -m gpu -q -x -p no:cacheprovider -k "non_finite or cache"
 echo "== alignment-sanitizer build of the emulated kernels (vector types alignas'd as on the device): the whole device suite"
 HK_EMULATE_KERNELS=1 HK_EMU_ALIGN=1 python -m pytest tests -m gpu -q -x -p no:cacheprovider
 echo "== a fresh random batch (seeds from the clock)"
