@@ -106,6 +106,13 @@ struct hk_context {
     cudaEvent_t ev_released = nullptr;
     bool released_recorded = false;
     Planes planes{};
+    // the light node's indirect pipeline runs on its own stream beside the sun and emissive ones (run_light), forked from and
+    // joined back into `stream` within the node, so every other ordering rule of the context only ever sees `stream`;
+    // it has its own scatter scratch, the other two share planes.scatter_*
+    cudaStream_t indirect_stream = nullptr;
+    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    uint32_t* indirect_scatter_key = nullptr;
+    ReservoirPlanes indirect_scatter_value{};
     bool noise_ready = false;
     bool planes_ready = false;         // allocate_planes completed: every pointer of `planes` is valid
     // TMA descriptors of kc_spatial's tiles (hk_tile.cuh): [0] indirect (radius 20, box 56), [1] emissive (radius 10, box 36);
@@ -379,6 +386,9 @@ static int allocate_planes(hk_context* ctx, uint32_t width, uint32_t height, uin
         for (int q = 0; q < 4; ++q) HK_CUDA(alloc_plane(ctx, &p.reservoir[r].q[q], n, L));
     HK_CUDA(alloc_plane(ctx, &p.scatter_key, n, L));   // zero = no claim; k_scatter_resolve re-zeroes what it consumes
     for (int q = 0; q < 4; ++q) HK_CUDA(alloc_plane(ctx, &p.scatter_value.q[q], n, L));
+    ctx->indirect_scatter_key = nullptr; ctx->indirect_scatter_value = ReservoirPlanes{};
+    HK_CUDA(alloc_plane(ctx, &ctx->indirect_scatter_key, n, L));
+    for (int q = 0; q < 4; ++q) HK_CUDA(alloc_plane(ctx, &ctx->indirect_scatter_value.q[q], n, L));
     HK_CUDA(alloc_plane(ctx, &p.tone_mapped_db[0], ctx->owned_pixels, L));
     HK_CUDA(alloc_plane(ctx, &p.tone_mapped_db[1], ctx->owned_pixels, L));
     p.tone_mapped = p.tone_mapped_db[0];
@@ -441,7 +451,15 @@ int hk_context_create_tile(hk_context** out, int cuda_device, uint32_t width, ui
         if (e != cudaSuccess) { delete c; return set_error(nullptr, HK_ERR_CUDA, cudaGetErrorString(e)); }
         c->own_stream = true;
     }
-    int rc = allocate_planes(c, width, height, col_begin, col_end, row_begin, row_end);
+    int rc = HK_OK;
+    {   // at the default priority, as the streams a host usually renders on: the block scheduler interleaves the two branches' CTAs
+        // freely (a higher priority for either branch measured slower, DESIGN.md §4a-6)
+        if (cudaStreamCreateWithFlags(&c->indirect_stream, cudaStreamNonBlocking) != cudaSuccess ||
+            cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess)
+            rc = set_error(c, HK_ERR_CUDA, "indirect light stream");
+    }
+    if (rc == HK_OK) rc = allocate_planes(c, width, height, col_begin, col_end, row_begin, row_end);
     if (rc == HK_OK) {
         void* p = nullptr;
         if (cudaMalloc(&p, sizeof(Counters)) != cudaSuccess) rc = set_error(c, HK_ERR_OUT_OF_MEMORY, "counters");
@@ -515,6 +533,9 @@ void hk_context_destroy(hk_context* ctx) {
         for (int j = 0; j < 2; ++j) if (ctx->kev[i][j]) cudaEventDestroy(ctx->kev[i][j]);
     for (int i = 0; i < hk_context::RING; ++i)
         for (int j = 0; j < 2; ++j) if (ctx->ring[i][j]) cudaEventDestroy(ctx->ring[i][j]);
+    if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
+    if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
+    if (ctx->indirect_stream) cudaStreamDestroy(ctx->indirect_stream);   // idle: its work is joined into `stream`, synchronised above
     if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
@@ -1357,18 +1378,18 @@ static int check_launch(hk_context* ctx) {
     return HK_OK;
 }
 
-struct KernelTimer {  // brackets one launch with events when pass timing is on
-    hk_context* c; int k;
-    KernelTimer(hk_context* ctx, int kernel) : c(ctx), k(kernel) {
+struct KernelTimer {  // brackets one launch (on `st`, the context's stream by default) with events when pass timing is on
+    hk_context* c; int k; cudaStream_t s;
+    KernelTimer(hk_context* ctx, int kernel, cudaStream_t st = nullptr) : c(ctx), k(kernel), s(st ? st : ctx->stream) {
         c->launches += 1;
         if (c->time_only >= 0) {
-            if (c->time_only == k && c->ring[0][0]) { cudaEventRecord(c->ring[c->ring_frames % hk_context::RING][0], c->stream); c->ring_hit = true; }
-        } else if (c->time_passes) { cudaEventRecord(c->kev[k][0], c->stream); c->kran[k] = true; }
+            if (c->time_only == k && c->ring[0][0]) { cudaEventRecord(c->ring[c->ring_frames % hk_context::RING][0], s); c->ring_hit = true; }
+        } else if (c->time_passes) { cudaEventRecord(c->kev[k][0], s); c->kran[k] = true; }
     }
     ~KernelTimer() {
         if (c->time_only >= 0) {
-            if (c->time_only == k && c->ring[0][0]) cudaEventRecord(c->ring[c->ring_frames % hk_context::RING][1], c->stream);
-        } else if (c->time_passes) cudaEventRecord(c->kev[k][1], c->stream);
+            if (c->time_only == k && c->ring[0][0]) cudaEventRecord(c->ring[c->ring_frames % hk_context::RING][1], s);
+        } else if (c->time_passes) cudaEventRecord(c->kev[k][1], s);
     }
 };
 
@@ -1384,15 +1405,38 @@ static int run_prepass(hk_context* ctx, KParams& P) {
 }
 static int ring_of(const KParams& P) { return P.tile_images ? RING_TONE : 0; }   // extra reach of every pass when a tile feeds the upscalers
 // spatial_reuse of one pipeline: the TMA-tiled kernel when descriptors exist and render space == G-buffer space, else the gather form
-static void launch_spatial(hk_context* ctx, const KParams& P, bool emissive) {
+static void launch_spatial(hk_context* ctx, const KParams& P, bool emissive, cudaStream_t st = nullptr) {
     const int v = emissive ? 1 : 0, parity = 1 - (int)(P.in.frame.number & 1u);
     const bool tiled = ctx->tile_maps_ready && ctx->tiled_spatial;
-    hk_launch_spatial(P, emissive, tiled ? &ctx->tm_depth[v] : nullptr, tiled ? &ctx->tm_q3[v][parity] : nullptr, ctx->spatial_tables_host[v], ctx->stream);
+    hk_launch_spatial(P, emissive, tiled ? &ctx->tm_depth[v] : nullptr, tiled ? &ctx->tm_q3[v][parity] : nullptr, ctx->spatial_tables_host[v],
+                      st ? st : ctx->stream);
 }
 static const TileMap* denoise_maps(hk_context* ctx, int level) { return (ctx->tile_maps_ready && ctx->tiled_denoise) ? ctx->tm_denoise[level] : nullptr; }
 static int run_light(hk_context* ctx, KParams& P) {  // LightNode::run order, light.rs:645-699 (albedo is fused in the prepass)
     const hk_frame_uniform& f = P.in.frame;
     const int GHOST_SPATIAL = ::GHOST_SPATIAL + ring_of(P);
+    // The three pipelines read the same G-buffer and write only their own signal's planes (DESIGN.md §4a-6).  The indirect one,
+    // with a scatter scratch of its own, runs on indirect_stream beside the sun and emissive ones: each branch's CTAs fill the SMs
+    // the other leaves idle while a kernel drains at a launch boundary.  Per-kernel pass timing keeps the serial order on one stream,
+    // so that each bracket holds one kernel alone.
+    const bool serial = ctx->time_passes && ctx->time_only < 0;
+    const cudaStream_t side = serial ? ctx->stream : ctx->indirect_stream;
+    KParams I = P;   // rows() rewrites the launch rectangle: each branch has its own copy
+    I.planes.scatter_key = ctx->indirect_scatter_key;
+    I.planes.scatter_value = ctx->indirect_scatter_value;
+    auto indirect = [&]() {
+        rows(ctx, I, GHOST_TEMPORAL + ctx->motion_margin);
+        { KernelTimer t(ctx, HK_K_INDIRECT, side);   // the per-pixel form's two kernels (path, then ReSTIR tail) count as one launch, as the pooled one
+          if (ctx->pooled_indirect) hk_launch_indirect_pool(I, f.indirect_bounces >= 2, ctx->count_rays, side);
+          else hk_launch_indirect(I, f.indirect_bounces >= 2, ctx->count_rays, wide_light(ctx), side);
+          hk_launch_scatter_resolve(I, 2, side); ctx->launches += 1; }
+        if (f.indirect_spatial_reuse) { rows(ctx, I, GHOST_SPATIAL); KernelTimer t(ctx, HK_K_INDIRECT_SPATIAL, side); launch_spatial(ctx, I, false, side); }
+    };
+    if (!serial) {
+        HK_CUDA(cudaEventRecord(ctx->ev_fork, ctx->stream));
+        HK_CUDA(cudaStreamWaitEvent(side, ctx->ev_fork, 0));
+        indirect();
+    }
     rows(ctx, P, GHOST_TEMPORAL + ctx->motion_margin);
     // each temporal pass is followed by the resolve of its scatter writes (all allocated rows can be targets)
     { KernelTimer t(ctx, HK_K_DIRECT); hk_launch_direct(P, false, ctx->count_rays, wide_light(ctx), ctx->stream);
@@ -1400,12 +1444,11 @@ static int run_light(hk_context* ctx, KParams& P) {  // LightNode::run order, li
     { KernelTimer t(ctx, HK_K_EMISSIVE); hk_launch_direct(P, true, ctx->count_rays, wide_light(ctx), ctx->stream);
       hk_launch_scatter_resolve(P, 1, ctx->stream); ctx->launches += 1; }
     if (f.emissive_spatial_reuse) { rows(ctx, P, GHOST_SPATIAL); KernelTimer t(ctx, HK_K_EMISSIVE_SPATIAL); launch_spatial(ctx, P, true); }
-    rows(ctx, P, GHOST_TEMPORAL + ctx->motion_margin);
-    { KernelTimer t(ctx, HK_K_INDIRECT);   // the per-pixel form's two kernels (path, then ReSTIR tail) count as one launch, as the pooled one
-      if (ctx->pooled_indirect) hk_launch_indirect_pool(P, f.indirect_bounces >= 2, ctx->count_rays, ctx->stream);
-      else hk_launch_indirect(P, f.indirect_bounces >= 2, ctx->count_rays, wide_light(ctx), ctx->stream);
-      hk_launch_scatter_resolve(P, 2, ctx->stream); ctx->launches += 1; }
-    if (f.indirect_spatial_reuse) { rows(ctx, P, GHOST_SPATIAL); KernelTimer t(ctx, HK_K_INDIRECT_SPATIAL); launch_spatial(ctx, P, false); }
+    if (serial) indirect();
+    else {   // join before the node returns: the post node, read-backs, scene updates and hk_sync order behind `stream` alone
+        HK_CUDA(cudaEventRecord(ctx->ev_join, side));
+        HK_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_join, 0));
+    }
     return check_launch(ctx);
 }
 // the kernels below overwrite the final images: a pipelined read-back of the previous frame must have left them first
