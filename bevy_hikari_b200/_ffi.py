@@ -63,6 +63,7 @@ SYMBOLS = {
     "hk_frame_read": (_I, [_P, _P, _P, _SZ]),
     "hk_upload_state": (_I, [_P, _I, _P, _SZ]),
     "hk_scene_update_transforms": (_I, [_P, _P, _P, _P, _U32]),
+    "hk_scene_add_meshes": (_I, [_P, _P, _U32, _P]),
     "hk_scene_readback": (_I, [_P, _I, _P, _SZ]),
     "hk_scene_buffer_bytes": (_I, [_P, _I, C.POINTER(_SZ)]),
     "hk_shared_scene_create": (_I, [C.POINTER(_P), _I, _P]),
@@ -70,6 +71,7 @@ SYMBOLS = {
     "hk_shared_scene_upload": (_I, [_P, C.POINTER(L.SceneDesc)]),
     "hk_shared_scene_update_instances": (_I, [_P, C.POINTER(L.SceneDesc)]),
     "hk_shared_scene_update_transforms": (_I, [_P, _P, _P, _P, _U32]),
+    "hk_shared_scene_add_meshes": (_I, [_P, _P, _U32, _P]),
     "hk_shared_scene_last_error": (C.c_char_p, [_P]),
     "hk_context_attach_scene": (_I, [_P, _P]),
     "hk_sync": (_I, [_P]),
@@ -93,6 +95,7 @@ SYMBOLS = {
     "hikari_world_create": (_P, []),
     "hikari_world_destroy": (None, [_P]),
     "hikari_world_add_mesh": (_U32, [_P, _P, _P, _P, _U32, _P, _U32, _U32]),
+    "hikari_world_add_device_mesh": (_U32, [_P, _P, _P, _P, _U32, _P, _U32, _U32]),
     "hikari_world_add_material": (_U32, [_P, _P]),
     "hikari_world_add_texture": (_U32, [_P, C.POINTER(L.TextureDesc)]),
     "hikari_world_add_instance": (_U32, [_P, _U32, _U32, _P, _U32]),
@@ -116,6 +119,7 @@ SYMBOLS = {
     "hikari_plugin_upload_scene": (_I, [_P, _P]),
     "hikari_plugin_update_instances": (_I, [_P, _P]),
     "hikari_plugin_update_transforms": (_I, [_P, _P, C.POINTER(_I)]),
+    "hikari_plugin_add_meshes": (_I, [_P, _P, _P, _U32, _P]),
     "hikari_plugin_run_frame": (_I, [_P, C.POINTER(Settings), C.POINTER(L.View), C.POINTER(L.PreviousView), C.POINTER(L.Lights)]),
     "hikari_plugin_context": (_P, [_P]),
     "hikari_plugin_frame_counter": (_U64, [_P]),
@@ -127,6 +131,7 @@ SYMBOLS = {
     "hikari_shared_scene_upload": (_I, [_P, _P]),
     "hikari_shared_scene_update_instances": (_I, [_P, _P]),
     "hikari_shared_scene_update_transforms": (_I, [_P, _P, C.POINTER(_I)]),
+    "hikari_shared_scene_add_meshes": (_I, [_P, _P, _P, _U32, _P]),
     "hikari_shared_scene_handle": (_P, [_P]),
     "hikari_plugin_attach_scene": (_I, [_P, _P]),
 }

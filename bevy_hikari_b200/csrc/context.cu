@@ -87,6 +87,10 @@ struct hk_shared_scene {
     std::vector<uint32_t> host_primitive_vertex_index;     // 3 per primitive (hk_primitive_vertex::index), same purpose
     std::vector<float> host_primitive_box;                 // 6 per primitive (min xyz, max xyz): what a BLAS leaf's navigator must enclose
     std::set<std::array<uint32_t, 4>> mesh_range_checked;   // hk_mesh_index values whose leaves have been validated
+    // the vertex, primitive and BLAS buffers as hk_scene_add_meshes grows them: those of the upload (scene_allocations, freed with
+    // them), then stream-ordered allocations of the scene's stream (`async`), replaced in stream order when they grow again.  The
+    // BLAS records past host_asset_nodes were built on the device and have no host copy (nor a 4-wide tree).
+    struct MeshBuf { void* p = nullptr; size_t cap = 0; bool async = false; } mbuf[3];
     DeviceScene scene{};
     bool ready = false;
     std::string error;
@@ -227,10 +231,35 @@ static void scene_end_write(hk_shared_scene* sc) {
 static void scene_before_free(hk_shared_scene* sc) {
     if (scene_cross(sc)) cudaStreamSynchronize(sc->stream);
 }
+// stream-ordered allocations on the scene's stream: hk_scene_add_meshes returns without waiting for the device, and a buffer it
+// replaces is released only after the frames in flight that read it (the emulation of tests/emu runs every launch synchronously)
+static cudaError_t malloc_on_stream(void** p, size_t bytes, cudaStream_t st) {
+#ifdef HK_EMU
+    (void)st;
+    return cudaMalloc(p, bytes);
+#else
+    return cudaMallocAsync(p, bytes, st);
+#endif
+}
+static void free_on_stream(void* p, cudaStream_t st) {
+#ifdef HK_EMU
+    (void)st;
+    cudaFree(p);
+#else
+    cudaFreeAsync(p, st);
+#endif
+}
+static void free_mesh_bufs(hk_shared_scene* sc) {      // (after the scene's stream is idle)
+    for (auto& b : sc->mbuf) {
+        if (b.async && b.p) cudaFree(b.p);
+        b = hk_shared_scene::MeshBuf();
+    }
+}
 static void scene_free(hk_shared_scene* sc) {
     cudaSetDevice(sc->device);
     if (sc->stream) cudaStreamSynchronize(sc->stream);
     free_list(sc->scene_allocations);
+    free_mesh_bufs(sc);
     for (auto& b : sc->ibuf) { if (b.p) cudaFree(b.p); b.p = nullptr; b.cap = 0; }
     for (auto& b : sc->pin) { if (b.p) cudaFreeHost(b.p); if (b.ev) cudaEventDestroy(b.ev); b = hk_shared_scene::PinBuf(); }
     if (sc->ev_ready) cudaEventDestroy(sc->ev_ready);
@@ -682,6 +711,7 @@ static int upload_wide(hk_shared_scene* sc, const hk_scene_desc* s, DeviceScene&
         std::vector<hk_shared_scene::WideMesh> meshes(keys.size());
         std::vector<uint32_t> prim_rank(sc->scene_primitive_count, 0u);
         for (size_t k = 0; k < keys.size(); ++k) {
+            if ((uint64_t)keys[k][0] + keys[k][1] > sc->host_asset_nodes.size()) continue;   // built on the device: no 4-wide tree
             const hk_node* flat = sc->host_asset_nodes.data() + keys[k][0];
             uint32_t shapes = 0;
             for (uint32_t r = 0; r < keys[k][1]; ++r)
@@ -734,6 +764,8 @@ static int upload_instances(hk_shared_scene* sc, const hk_scene_desc* s, DeviceS
         const std::array<uint32_t, 4> mesh_key = {in.mesh.vertex, in.mesh.primitive, in.mesh.node_offset, in.mesh.node_count};
         if (!sc->mesh_range_checked.count(mesh_key)) {
             const std::vector<hk_node>& nodes = sc->host_asset_nodes;
+            if ((uint64_t)in.mesh.node_offset + in.mesh.node_count > nodes.size())     // records built on the device: only as added
+                return set_error(sc, HK_ERR_INVALID_ARGUMENT, "instance references a BLAS range that is not one hk_scene_add_meshes returned");
             for (uint32_t k = 0; k < in.mesh.node_count; ++k) {
                 const hk_node& nd = nodes[in.mesh.node_offset + k];
                 if (nd.entry_index >= 0x80000000u) {
@@ -903,6 +935,7 @@ static int scene_upload(hk_shared_scene* sc, const hk_scene_desc* s) {
     HK_SCUDA(cudaSetDevice(sc->device));
     HK_SCUDA(cudaStreamSynchronize(sc->stream));     // (after scene_begin_write: also every attached camera's last read)
     free_list(sc->scene_allocations);
+    free_mesh_bufs(sc);
     sc->ready = false;
     sc->mesh_boxes_match = boxes_match;
     sc->scene_material_count = 0;
@@ -930,6 +963,9 @@ static int scene_upload(hk_shared_scene* sc, const hk_scene_desc* s) {
     HK_SCUDA(upload(sc, &d.vertices, s->vertices, s->vertex_count));
     HK_SCUDA(upload(sc, &d.primitives, s->primitives, s->primitive_count));
     HK_SCUDA(upload(sc, &d.asset_nodes, s->asset_nodes, s->asset_node_count));
+    sc->mbuf[0] = {const_cast<hk_vertex*>(d.vertices), sizeof(hk_vertex) * (size_t)s->vertex_count, false};
+    sc->mbuf[1] = {const_cast<hk_primitive*>(d.primitives), sizeof(hk_primitive) * (size_t)s->primitive_count, false};
+    sc->mbuf[2] = {const_cast<hk_node*>(d.asset_nodes), sizeof(hk_node) * (size_t)s->asset_node_count, false};
     d.materials = nullptr;           // uploaded with the per-frame half below
     d.texture_count = s->texture_count;
     d.textures = nullptr;
@@ -990,6 +1026,23 @@ static bool wide_primary(const hk_context* ctx);
 static bool wide_light(const hk_context* ctx);
 }
 
+// The next of the scene's two pinned staging slots with room for `bytes`; waits only for the copy made from it two calls ago.
+// The caller records pin.ev after its copy and sets pin.used.
+static int pinned_slot(hk_shared_scene* sc, size_t bytes, hk_shared_scene::PinBuf** out) {
+    hk_shared_scene::PinBuf& pin = sc->pin[sc->pin_slot];
+    sc->pin_slot ^= 1;
+    if (!pin.ev) HK_SCUDA(cudaEventCreateWithFlags(&pin.ev, cudaEventDisableTiming));
+    if (pin.used) HK_SCUDA(cudaEventSynchronize(pin.ev));          // the copy made from this slot two calls ago
+    if (pin.cap < bytes) {
+        if (pin.p) cudaFreeHost(pin.p);
+        pin.p = nullptr; pin.cap = 0;
+        HK_SCUDA(cudaMallocHost(&pin.p, bytes + bytes / 2));
+        pin.cap = bytes + bytes / 2;
+    }
+    *out = &pin;
+    return HK_OK;
+}
+
 // SURVEY 8(f) rank 2 — the per-frame half of the scene rebuilt on the device (kernels_scene.cu) from the model matrices alone.
 static int scene_update_transforms(hk_shared_scene* sc, const float* models, const float* previous_models, const float* mesh_aabbs,
                                    uint32_t instance_count, uint32_t* launches) {
@@ -1017,16 +1070,9 @@ static int scene_update_transforms(hk_shared_scene* sc, const float* models, con
     const size_t mbytes = 64u * (size_t)n, abytes = 24u * (size_t)n;
     const size_t stage_bytes = mbytes * (previous_models ? 2u : 1u) + abytes;
     // pinned staging: the caller's arrays are free on return and the host does not wait for the frames in flight
-    hk_shared_scene::PinBuf& pin = sc->pin[sc->pin_slot];
-    sc->pin_slot ^= 1;
-    if (!pin.ev) HK_SCUDA(cudaEventCreateWithFlags(&pin.ev, cudaEventDisableTiming));
-    if (pin.used) HK_SCUDA(cudaEventSynchronize(pin.ev));          // the copy made from this slot two calls ago
-    if (pin.cap < stage_bytes) {
-        if (pin.p) cudaFreeHost(pin.p);
-        pin.p = nullptr; pin.cap = 0;
-        HK_SCUDA(cudaMallocHost(&pin.p, stage_bytes + stage_bytes / 2));
-        pin.cap = stage_bytes + stage_bytes / 2;
-    }
+    hk_shared_scene::PinBuf* slot = nullptr;
+    if (const int rc = pinned_slot(sc, stage_bytes, &slot)) return rc;
+    hk_shared_scene::PinBuf& pin = *slot;
     // staging layout: models | previous models (optional) | mesh AABBs — the two matrix arrays are read as float4 and must stay
     // 16-byte aligned for every n (24 n bytes of AABBs in between misaligned `previous` for odd n: a misaligned-address fault on
     // the device that the host emulation did not see)
@@ -1088,6 +1134,141 @@ static int scene_update_transforms(hk_shared_scene* sc, const float* models, con
     return HK_OK;
 }
 
+// SURVEY 8(f) rank 2, the meshes: GpuMesh::try_from for meshes added to a live scene, on the device (kernels_scene.cu).  Everything
+// the kernels rely on is checked here first, in one pass over the caller's arrays, so that a refused call launches nothing and
+// leaves the scene as it was.
+static int scene_add_meshes(hk_shared_scene* sc, const hk_mesh_source* meshes, uint32_t n, hk_mesh_index* out, uint32_t* launches) {
+    if (!sc->ready) return set_error(sc, HK_ERR_NOT_READY, "hk_scene_add_meshes needs a scene from hk_scene_upload");
+    if (n == 0u) return HK_OK;
+    std::vector<MeshJob> jobs(n);
+    std::vector<hk_mesh_index> index(n);
+    uint64_t nv_total = 0, np_total = 0, ni_total = 0, nodes_total = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        const hk_mesh_source& m = meshes[i];
+        auto refuse = [&](const std::string& why) {
+            return set_error(sc, HK_ERR_INVALID_ARGUMENT, "hk_scene_add_meshes: mesh " + std::to_string(i) + ": " + why);
+        };
+        if (!m.positions || !m.position_count) return refuse("MissingAttribute(ATTRIBUTE_POSITION)");      // mod.rs:301-308
+        if (!m.normals || !m.normal_count) return refuse("MissingAttribute(ATTRIBUTE_NORMAL)");
+        if (!m.uvs || !m.uv_count) return refuse("MissingAttribute(ATTRIBUTE_UV_0)");
+        if (m.topology != HK_TOPOLOGY_TRIANGLE_LIST && m.topology != HK_TOPOLOGY_TRIANGLE_STRIP)
+            return refuse("IncompatiblePrimitiveTopology (topology " + std::to_string(m.topology) + ")");
+        const uint32_t nv = std::min(m.position_count, std::min(m.normal_count, m.uv_count));     // multizip
+        const bool strip = m.topology == HK_TOPOLOGY_TRIANGLE_STRIP, indexed = m.indices != nullptr;
+        const uint64_t ni = indexed ? m.index_count : nv;
+        if (!strip && ni % 3u != 0u) return refuse("IncompatiblePrimitiveTopology (a short chunk: " + std::to_string(ni) + " indices in a triangle list)");
+        const uint64_t np = strip ? (ni >= 3u ? ni - 2u : 0u) : ni / 3u;
+        if (np == 0u) return refuse("NoPrimitive");
+        if (np >= 0x80000000ull) return refuse(std::to_string(np) + " primitives do not fit the BLAS leaf flag (0x80000000)");
+        if (indexed)
+            for (uint32_t k = 0; k < m.index_count; ++k)
+                if (m.indices[k] >= nv)
+                    return refuse("index " + std::to_string(k) + " = " + std::to_string(m.indices[k]) + " is not below the vertex count " + std::to_string(nv));
+        const uint64_t nodes = np == 1u ? 1u : 3u * np - 2u;
+        const uint64_t v0 = (uint64_t)sc->scene_vertex_count + nv_total, p0 = (uint64_t)sc->scene_primitive_count + np_total;
+        const uint64_t n0 = (uint64_t)sc->scene_asset_node_count + nodes_total;
+        if (v0 + nv > 0xFFFFFFFFull || p0 + np > 0xFFFFFFFFull || n0 + nodes > 0xFFFFFFFFull || ni_total + (indexed ? ni : 0u) > 0xFFFFFFFFull)
+            return refuse("the scene's vertex / primitive / BLAS record offsets would not fit 32 bits");
+        index[i] = hk_mesh_index{(uint32_t)v0, (uint32_t)p0, (uint32_t)n0, (uint32_t)nodes};
+        jobs[i] = MeshJob{(uint32_t)nv_total, (uint32_t)ni_total, indexed ? 1u : 0u, strip ? 1u : 0u, (uint32_t)np_total, (uint32_t)np,
+                          (uint32_t)v0, (uint32_t)p0, (uint32_t)n0};
+        nv_total += nv; np_total += np; nodes_total += nodes;
+        if (indexed) ni_total += ni;
+    }
+    HK_SCUDA(cudaSetDevice(sc->device));
+    // staging: jobs | positions | normals | uvs | indices, each 16-byte aligned
+    auto align16 = [](size_t x) { return (x + 15u) & ~(size_t)15u; };
+    const size_t o_pos = align16(sizeof(MeshJob) * (size_t)n), o_nrm = o_pos + align16(12u * nv_total), o_uv = o_nrm + align16(12u * nv_total);
+    const size_t o_idx = o_uv + align16(8u * nv_total), stage_bytes = o_idx + align16(4u * ni_total);
+    hk_shared_scene::PinBuf* slot = nullptr;
+    if (const int rc = pinned_slot(sc, stage_bytes, &slot)) return rc;
+    uint8_t* hp = static_cast<uint8_t*>(slot->p);
+    memcpy(hp, jobs.data(), sizeof(MeshJob) * (size_t)n);
+    for (uint32_t i = 0; i < n; ++i) {
+        const hk_mesh_source& m = meshes[i];
+        const MeshJob& j = jobs[i];
+        const size_t nv = (i + 1u < n ? jobs[i + 1u].src_vertex : nv_total) - j.src_vertex;
+        memcpy(hp + o_pos + 12u * (size_t)j.src_vertex, m.positions, 12u * nv);
+        memcpy(hp + o_nrm + 12u * (size_t)j.src_vertex, m.normals, 12u * nv);
+        memcpy(hp + o_uv + 8u * (size_t)j.src_vertex, m.uvs, 8u * nv);
+        if (j.indexed) memcpy(hp + o_idx + 4u * (size_t)j.src_index, m.indices, 4u * (size_t)m.index_count);
+    }
+    // the scene's buffers, grown where needed: a new allocation takes the records the frames read so far, in stream order.  Every
+    // allocation is made before anything is copied or released, so that a failed one leaves the scene on its old buffers.
+    const size_t rec[3] = {sizeof(hk_vertex), sizeof(hk_primitive), sizeof(hk_node)};
+    const uint64_t have[3] = {sc->scene_vertex_count, sc->scene_primitive_count, sc->scene_asset_node_count};
+    const uint64_t add[3] = {nv_total, np_total, nodes_total};
+    size_t need[3], cap[3];
+    void* grown[3] = {nullptr, nullptr, nullptr};
+    void* block = nullptr;       // staged copy + build scratch, released in stream order behind the build
+    const size_t scratch_off = align16(stage_bytes);
+    cudaError_t e = malloc_on_stream(&block, scratch_off + hk_blas_scratch_bytes((uint32_t)np_total), sc->stream);
+    for (int b = 0; b < 3 && e == cudaSuccess; ++b) {
+        need[b] = rec[b] * (size_t)(have[b] + add[b]) + 64u;        // +64: 16-byte vector loads at the tail stay in bounds
+        cap[b] = need[b] + need[b] / 2u;
+        if (sc->mbuf[b].cap < need[b]) e = malloc_on_stream(&grown[b], cap[b], sc->stream);
+    }
+    if (e != cudaSuccess) {
+        for (void* p : grown) if (p) free_on_stream(p, sc->stream);
+        if (block) free_on_stream(block, sc->stream);
+        HK_SCUDA(e);
+    }
+    void* retired[3] = {nullptr, nullptr, nullptr};      // released behind the build, once the new pointers are published
+    for (int b = 0; b < 3; ++b) {
+        if (!grown[b]) continue;
+        hk_shared_scene::MeshBuf& mb = sc->mbuf[b];
+        HK_SCUDA(cudaMemcpyAsync(grown[b], mb.p, rec[b] * (size_t)have[b], cudaMemcpyDeviceToDevice, sc->stream));
+        HK_SCUDA(cudaMemsetAsync(static_cast<uint8_t*>(grown[b]) + need[b] - 64u, 0, 64u, sc->stream));
+        if (mb.async) retired[b] = mb.p;      // an upload's buffer goes with the upload's allocations
+        mb = hk_shared_scene::MeshBuf{grown[b], cap[b], true};
+    }
+    uint8_t* dp = static_cast<uint8_t*>(block);
+    HK_SCUDA(cudaMemcpyAsync(dp, hp, stage_bytes, cudaMemcpyHostToDevice, sc->stream));
+    HK_SCUDA(cudaEventRecord(slot->ev, sc->stream));
+    slot->used = true;
+    hk_vertex* vertices = static_cast<hk_vertex*>(sc->mbuf[0].p);
+    hk_primitive* primitives = static_cast<hk_primitive*>(sc->mbuf[1].p);
+    hk_node* nodes = static_cast<hk_node*>(sc->mbuf[2].p);
+    *launches = (uint32_t)hk_launch_build_meshes(n, reinterpret_cast<const MeshJob*>(dp), (uint32_t)nv_total, (uint32_t)np_total,
+                                                  reinterpret_cast<const float*>(dp + o_pos), reinterpret_cast<const float*>(dp + o_nrm),
+                                                  reinterpret_cast<const float*>(dp + o_uv), reinterpret_cast<const uint32_t*>(dp + o_idx),
+                                                  dp + scratch_off, vertices, primitives, nodes, sc->stream);
+    HK_SCUDA(cudaGetLastError());
+    free_on_stream(block, sc->stream);
+    // host copies that validate later instance updates; the new BLAS ranges are checked by construction
+    sc->host_primitive_vertex_index.resize(3u * (size_t)(sc->scene_primitive_count + np_total));
+    sc->host_primitive_box.resize(6u * (size_t)(sc->scene_primitive_count + np_total));
+    for (uint32_t i = 0; i < n; ++i) {
+        const hk_mesh_source& m = meshes[i];
+        const MeshJob& j = jobs[i];
+        for (uint32_t p = 0; p < j.shapes; ++p) {
+            uint32_t id[3];
+            for (uint32_t k = 0; k < 3u; ++k) {
+                const uint32_t at = j.strip ? p + k : 3u * p + k;
+                id[k] = j.indexed ? m.indices[at] : at;
+            }
+            if (j.strip && (p & 1u)) std::swap(id[0], id[1]);
+            const size_t g = (size_t)j.dst_primitive + p;
+            for (int c = 0; c < 3; ++c) {
+                sc->host_primitive_vertex_index[3u * g + c] = id[c];
+                const float a = m.positions[3u * (size_t)id[0] + c], b = m.positions[3u * (size_t)id[1] + c], e = m.positions[3u * (size_t)id[2] + c];
+                sc->host_primitive_box[6u * g + c] = fminf(a, fminf(b, e));
+                sc->host_primitive_box[6u * g + 3u + c] = fmaxf(a, fmaxf(b, e));
+            }
+        }
+        sc->mesh_range_checked.insert({index[i].vertex, index[i].primitive, index[i].node_offset, index[i].node_count});
+        out[i] = index[i];
+    }
+    sc->scene_vertex_count += (uint32_t)nv_total;
+    sc->scene_primitive_count += (uint32_t)np_total;
+    sc->scene_asset_node_count += (uint32_t)nodes_total;
+    DeviceScene d = sc->scene;          // published behind the launches above: frames enqueued from now on read the grown buffers
+    d.vertices = vertices; d.primitives = primitives; d.asset_nodes = nodes;
+    sc->scene = d;
+    for (void* p : retired) if (p) free_on_stream(p, sc->stream);
+    return HK_OK;
+}
+
 // {ready, stack need, TLAS node count} of the scene's 4-wide TLAS.  After a derivation on the device they exist only there
 // and are read back: a query (hk_get_stats, hk_scene_readback), not a frame call, so it may wait for the scene's stream.
 static cudaError_t wide_tlas_state(hk_shared_scene* sc, uint32_t out[3]) {
@@ -1118,6 +1299,9 @@ static bool scene_buffer(hk_shared_scene* sc, int which, const void** src, size_
         case HK_SCENE_EMISSIVE_NODES: *src = d.emissive_nodes; *have = sizeof(hk_node) * (size_t)d.emissive_node_count; return true;
         case HK_SCENE_PREVIOUS_MODELS: *src = d.previous_models; *have = d.previous_models ? 64u * (size_t)sc->scene_instance_count : 0u; return true;
         case HK_SCENE_INSTANCE_MOVED: *src = d.instance_moved; *have = d.instance_moved ? 4u * (size_t)sc->scene_instance_count : 0u; return true;
+        case HK_SCENE_VERTICES: *src = d.vertices; *have = sizeof(hk_vertex) * (size_t)sc->scene_vertex_count; return true;
+        case HK_SCENE_PRIMITIVES: *src = d.primitives; *have = sizeof(hk_primitive) * (size_t)sc->scene_primitive_count; return true;
+        case HK_SCENE_ASSET_NODES: *src = d.asset_nodes; *have = sizeof(hk_node) * (size_t)sc->scene_asset_node_count; return true;
         default: return false;
     }
 }
@@ -1164,6 +1348,13 @@ static int do_update_transforms(hk_shared_scene* sc, const float* models, const 
     scene_end_write(sc);
     return rc;
 }
+static int do_add_meshes(hk_shared_scene* sc, const hk_mesh_source* meshes, uint32_t n, hk_mesh_index* out, uint32_t* launches) {
+    if (!sc->ready) return set_error(sc, HK_ERR_NOT_READY, "hk_scene_add_meshes needs a scene from hk_scene_upload");
+    scene_begin_write(sc);
+    const int rc = scene_add_meshes(sc, meshes, n, out, launches);
+    scene_end_write(sc);
+    return rc;
+}
 
 extern "C" {
 
@@ -1190,6 +1381,18 @@ int hk_scene_update_transforms(hk_context* ctx, const float* models, const float
     if (!sc) return set_error(ctx, HK_ERR_NOT_READY, "hk_scene_update_transforms needs a scene from hk_scene_upload");
     uint32_t launches = 0;
     rc = scene_result(ctx, sc, do_update_transforms(sc, models, previous_models, mesh_aabbs, instance_count, &launches));
+    ctx->launches += launches;
+    return rc;
+}
+
+int hk_scene_add_meshes(hk_context* ctx, const hk_mesh_source* meshes, uint32_t mesh_count, hk_mesh_index* out) {
+    if (!ctx || (mesh_count && (!meshes || !out))) return HK_ERR_INVALID_ARGUMENT;
+    hk_shared_scene* sc = nullptr;
+    int rc = private_scene(ctx, false, &sc);
+    if (rc != HK_OK) return rc;
+    if (!sc) return set_error(ctx, HK_ERR_NOT_READY, "hk_scene_add_meshes needs a scene from hk_scene_upload");
+    uint32_t launches = 0;
+    rc = scene_result(ctx, sc, do_add_meshes(sc, meshes, mesh_count, out, &launches));
     ctx->launches += launches;
     return rc;
 }
@@ -1234,6 +1437,11 @@ int hk_shared_scene_update_transforms(hk_shared_scene* sc, const float* models, 
     if (!sc || (instance_count && (!models || !mesh_aabbs))) return HK_ERR_INVALID_ARGUMENT;
     uint32_t launches = 0;
     return do_update_transforms(sc, models, previous_models, mesh_aabbs, instance_count, &launches);
+}
+int hk_shared_scene_add_meshes(hk_shared_scene* sc, const hk_mesh_source* meshes, uint32_t mesh_count, hk_mesh_index* out) {
+    if (!sc || (mesh_count && (!meshes || !out))) return HK_ERR_INVALID_ARGUMENT;
+    uint32_t launches = 0;
+    return do_add_meshes(sc, meshes, mesh_count, out, &launches);
 }
 const char* hk_shared_scene_last_error(hk_shared_scene* sc) { return sc ? sc->error.c_str() : g_create_error.c_str(); }
 

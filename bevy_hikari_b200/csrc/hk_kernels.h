@@ -51,5 +51,19 @@ size_t hk_scene_bvh_scratch_bytes(uint32_t n);
 void hk_launch_build_wide_tlas(uint32_t n, const hk_node* flat, bool blas_ok, uint32_t base_need, void* scratch, hkd::hk_wide_node* nodes,
                                uint32_t* rank, uint32_t* state, cudaStream_t st);
 size_t hk_wide_tlas_scratch_bytes(uint32_t n);
+// GpuMesh::try_from (mod.rs:379-467) on the device for a batch of meshes (hk_scene_add_meshes): per mesh, where its staged
+// attributes and indices start, which topology it has, and where its records go in the scene's buffers.  Shapes (primitives) are
+// numbered across the batch; jobs are in batch order.
+struct MeshJob {
+    uint32_t src_vertex, src_index, indexed, strip;        // staged positions / normals / uvs from src_vertex, indices from src_index
+    uint32_t shape_begin, shapes;                           // the mesh's primitives in the batch
+    uint32_t dst_vertex, dst_primitive, dst_node;           // first record in the scene's vertex / primitive / BLAS buffers
+};
+// packs the vertices and primitives of the batch and builds every mesh's BLAS (bvh 0.7.1, as host/hikari.cpp build_flat_bvh with no
+// node-index write-back) into nodes[dst_node ..); `scratch`: hk_blas_scratch_bytes(total_primitives).  Returns the launch count.
+int hk_launch_build_meshes(uint32_t n_jobs, const MeshJob* jobs, uint32_t total_vertices, uint32_t total_primitives, const float* positions,
+                           const float* normals, const float* uvs, const uint32_t* indices, void* scratch, hk_vertex* vertices,
+                           hk_primitive* primitives, hk_node* nodes, cudaStream_t st);
+size_t hk_blas_scratch_bytes(uint32_t primitives);
 void hk_launch_scene_emissives(uint32_t ne, hk_emissive* emissives, const hk_instance* instances, const hk_material* materials,
                                const hk_primitive* primitives, const hk_vertex* vertices, float4* box_lo, float4* box_hi, cudaStream_t st);

@@ -24,7 +24,12 @@
 //                        (tests/test_gpu_wide_tlas_device.py holds it to the host derivation)
 // What this path does NOT rebuild: alias tables (their cache rule — rebuild when the scale moved by more than 0.01,
 // instance.rs:385-397 — is the caller's to check: hikari::MeshMaterialWorld::prepare_instance_transforms) and anything that changes
-// the SET of instances, meshes or materials; those go through hk_scene_update_instances / hk_scene_upload.
+// the SET of instances or materials; those go through hk_scene_update_instances / hk_scene_upload.
+// Meshes added to the scene (hk_scene_add_meshes) are built here too — GpuMesh::try_from of mod.rs:379-467, see "mesh assets" below:
+//   k_mesh_records       one thread per vertex and per primitive: the records, each primitive's box and centre
+//   kc_build_blas_top    one CTA per mesh: the top levels of its BLAS, the whole CTA on one node
+//   kc_build_blas_bottom the subtrees below, taken from a work list, one warp per node
+// with the same split routine (sah_split) as kc_build_flat_bvh.  Changing or removing an existing mesh is not done.
 #include "hk_device.cuh"
 #include "hk_wide.cuh"
 #include "hk_kernels.h"
@@ -71,10 +76,6 @@ __device__ __forceinline__ uint32_t warp_sum(uint32_t v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
-}
-__device__ __forceinline__ void warp_join(SBox& b) {
-#pragma unroll
-    for (int k = 0; k < 3; ++k) { b.mn[k] = warp_min(b.mn[k]); b.mx[k] = warp_max(b.mx[k]); }
 }
 
 __device__ __forceinline__ void store_node(hk_node* out, uint32_t at, const SBox& b, uint32_t entry, uint32_t exit) {
@@ -211,26 +212,341 @@ __global__ void __launch_bounds__(128) k_scene_instances(uint32_t n, const float
 }
 
 // ------------------------------------------------------------------------------------------------ SAH build + flatten
-// One tree node of the level being split.  `t` = its index among the tree nodes in pre-order (what bvh calls the node index and
-// writes back through set_bh_node_index), `leaves_before` = shapes that precede it in pre-order; its navigator record sits at
-// t - 1 + leaves_before (the root has none).
+// One tree node being split.  `t` = its index among the tree nodes in pre-order (what bvh calls the node index and writes back
+// through set_bh_node_index), `leaves_before` = shapes that precede it in pre-order; its navigator record sits at
+// t - 1 + leaves_before (the root has none).  Each node writes its own navigator: the box bvh gives a child (l_box / r_box of
+// BVH::build) is the join of the child's shapes in the order the child holds them, which is the child's own bound, except when no
+// SAH candidate had a cost below infinity (NaN or infinite costs): then the parent leaves both children the empty box.
+constexpr uint32_t SEG_EMPTY_BOX = 1u;     // BuildSeg::flags: the navigator gets the empty box
+constexpr uint32_t SEG_IDX_B = 2u;         // the segment's shape list is in idx_b (else idx_a)
 struct BuildSeg {
-    uint32_t begin, count, t, leaves_before;
-    float lo[3], hi[3];          // the box the PARENT computed for this child (l_box / r_box of BVH::build)
+    uint32_t begin, count, t, leaves_before, flags, mesh;     // mesh: the BLAS job of a kc_build_blas_* segment (0 for the TLAS)
 };
-static_assert(sizeof(BuildSeg) == 40, "scratch sizing in context.cu");
+static_assert(sizeof(BuildSeg) == 24, "scratch sizing below");
 
+// What one split needs: the shapes' boxes and centres (indexed by shape), the two shape lists, and where the records go.
+struct BuildIn {
+    const float4 *box_lo, *box_hi, *center;
+    uint32_t* idx[2];
+    hk_node* out;                 // the flat array of this tree
+    uint32_t shape_base;          // leaf records name shape - shape_base
+    uint8_t* index_base;          // per shape: its node index t is written at index_base + shape * index_stride (nullptr: none)
+    uint32_t index_stride;
+};
+
+// bvh 0.7.1's bucket of a centre: Rust's saturating `f32 as usize`, clamped to the last bucket as host/hikari.cpp clamps it
+__device__ __forceinline__ uint32_t sah_bucket(float rel) {
+    const float x = rel * ((float)SCENE_BUCKETS - 0.01f);
+    if (!(x > 0.0f)) return 0u;
+    if (x >= (float)SCENE_BUCKETS) return (uint32_t)SCENE_BUCKETS - 1u;
+    const uint32_t b = (uint32_t)x;
+    return b < (uint32_t)SCENE_BUCKETS ? b : (uint32_t)SCENE_BUCKETS - 1u;
+}
+__device__ __forceinline__ float4 box_center(const float4 lo, const float4 hi) {      // AABB::center
+    return make_float4(lo.x + (hi.x - lo.x) / 2.0f, lo.y + (hi.y - lo.y) / 2.0f, lo.z + (hi.z - lo.z) / 2.0f, 0.0f);
+}
+
+// The join of boxes in a given order, bit for bit.  min / max over the values do not depend on the order (a NaN never wins against
+// the running bound, which starts at +-inf and so is never NaN); the one thing that does is which zero a bound of 0 keeps, -0 or +0:
+// the first zero in the order.  So each bound also carries (position << 1 | sign) of the first zero it met.
+struct OrderedBox {
+    SBox b;
+    uint32_t z[6];
+    __device__ __forceinline__ void clear() {
+        b.clear();
+#pragma unroll
+        for (int k = 0; k < 6; ++k) z[k] = 0xFFFFFFFFu;
+    }
+    __device__ __forceinline__ void add(uint32_t pos, const float4 lo, const float4 hi) {
+        const float l[3] = {lo.x, lo.y, lo.z}, h[3] = {hi.x, hi.y, hi.z};
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            b.mn[k] = smin(b.mn[k], l[k]); b.mx[k] = smax(b.mx[k], h[k]);
+            if (l[k] == 0.0f && z[k] == 0xFFFFFFFFu) z[k] = pos << 1 | (__float_as_uint(l[k]) >> 31);
+            if (h[k] == 0.0f && z[3 + k] == 0xFFFFFFFFu) z[3 + k] = pos << 1 | (__float_as_uint(h[k]) >> 31);
+        }
+    }
+    __device__ __forceinline__ void settle_zeros() {       // after the reduction over the team
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            if (b.mn[k] == 0.0f) b.mn[k] = (z[k] & 1u) ? -0.0f : 0.0f;
+            if (b.mx[k] == 0.0f) b.mx[k] = (z[3 + k] & 1u) ? -0.0f : 0.0f;
+        }
+    }
+};
+
+// A team of threads that splits one node together: a warp (the TLAS, and a BLAS below the top levels) or a whole CTA (the top
+// levels of a large BLAS).  reduce() combines per-thread values in place (mins, maxs, unsigned mins, sums); ranks() gives each
+// thread's position in a stable counting sort of one round of `size` elements by bucket (SCENE_BUCKETS = no element).
+struct WarpTeam {
+    uint32_t lane;
+    __device__ __forceinline__ uint32_t rank() const { return lane; }
+    __device__ __forceinline__ uint32_t size() const { return 32u; }
+    template <int NF, int NX, int NU, int NS>
+    __device__ __forceinline__ void reduce(float* mins, float* maxs, uint32_t* umins, uint32_t* sums) {
+#pragma unroll
+        for (int i = 0; i < NF; ++i) mins[i] = warp_min(mins[i]);
+#pragma unroll
+        for (int i = 0; i < NX; ++i) maxs[i] = warp_max(maxs[i]);
+#pragma unroll
+        for (int i = 0; i < NU; ++i)
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) umins[i] = min(umins[i], __shfl_xor_sync(0xffffffffu, umins[i], o));
+#pragma unroll
+        for (int i = 0; i < NS; ++i) sums[i] = warp_sum(sums[i]);
+    }
+    __device__ __forceinline__ uint32_t ranks(uint32_t bucket, uint32_t* off) {
+        const uint32_t lt = (1u << lane) - 1u;
+        uint32_t pos = 0u;
+#pragma unroll
+        for (int b = 0; b < SCENE_BUCKETS; ++b) {
+            const uint32_t mask = __ballot_sync(0xffffffffu, bucket == (uint32_t)b);
+            if (bucket == (uint32_t)b) pos = off[b] + (uint32_t)__popc(mask & lt);
+            off[b] += (uint32_t)__popc(mask);
+        }
+        return pos;
+    }
+};
+
+constexpr int CTA_TEAM_SLOTS = 48;         // the most values one reduce() combines (the buckets: 18 + 18 + 6)
+struct CtaTeamShared {
+    uint32_t red[32][CTA_TEAM_SLOTS];
+    uint32_t cnt[SCENE_BUCKETS][32];
+};
+struct CtaTeam {
+    CtaTeamShared* sh;
+    uint32_t tid, warps;
+    __device__ __forceinline__ uint32_t rank() const { return tid; }
+    __device__ __forceinline__ uint32_t size() const { return warps * 32u; }
+    template <int NF, int NX, int NU, int NS>
+    __device__ void reduce(float* mins, float* maxs, uint32_t* umins, uint32_t* sums) {
+        static_assert(NF + NX + NU + NS <= CTA_TEAM_SLOTS, "CtaTeamShared::red");
+        WarpTeam w{tid & 31u};
+        w.reduce<NF, NX, NU, NS>(mins, maxs, umins, sums);
+        const uint32_t warp = tid >> 5;
+        if ((tid & 31u) == 0u) {
+#pragma unroll
+            for (int i = 0; i < NF; ++i) sh->red[warp][i] = __float_as_uint(mins[i]);
+#pragma unroll
+            for (int i = 0; i < NX; ++i) sh->red[warp][NF + i] = __float_as_uint(maxs[i]);
+#pragma unroll
+            for (int i = 0; i < NU; ++i) sh->red[warp][NF + NX + i] = umins[i];
+#pragma unroll
+            for (int i = 0; i < NS; ++i) sh->red[warp][NF + NX + NU + i] = sums[i];
+        }
+        __syncthreads();
+#pragma unroll
+        for (int i = 0; i < NF; ++i) { float v = mins[i]; for (uint32_t q = 0; q < warps; ++q) v = smin(v, __uint_as_float(sh->red[q][i])); mins[i] = v; }
+#pragma unroll
+        for (int i = 0; i < NX; ++i) { float v = maxs[i]; for (uint32_t q = 0; q < warps; ++q) v = smax(v, __uint_as_float(sh->red[q][NF + i])); maxs[i] = v; }
+#pragma unroll
+        for (int i = 0; i < NU; ++i) { uint32_t v = umins[i]; for (uint32_t q = 0; q < warps; ++q) v = min(v, sh->red[q][NF + NX + i]); umins[i] = v; }
+#pragma unroll
+        for (int i = 0; i < NS; ++i) { uint32_t v = 0u; for (uint32_t q = 0; q < warps; ++q) v += sh->red[q][NF + NX + NU + i]; sums[i] = v; }
+        __syncthreads();
+    }
+    __device__ uint32_t ranks(uint32_t bucket, uint32_t* off) {
+        const uint32_t lane = tid & 31u, warp = tid >> 5, lt = (1u << lane) - 1u;
+        uint32_t in_warp = 0u;
+#pragma unroll
+        for (int b = 0; b < SCENE_BUCKETS; ++b) {
+            const uint32_t mask = __ballot_sync(0xffffffffu, bucket == (uint32_t)b);
+            if (bucket == (uint32_t)b) in_warp = (uint32_t)__popc(mask & lt);
+            if (lane == 0u) sh->cnt[b][warp] = (uint32_t)__popc(mask);
+        }
+        __syncthreads();
+        uint32_t pos = 0u;
+#pragma unroll
+        for (int b = 0; b < SCENE_BUCKETS; ++b) {
+            uint32_t before = 0u, total = 0u;
+            for (uint32_t q = 0; q < warps; ++q) {
+                const uint32_t c = sh->cnt[b][q];
+                before += q < warp ? c : 0u;
+                total += c;
+            }
+            if (bucket == (uint32_t)b) pos = off[b] + before + in_warp;
+            off[b] += total;
+        }
+        __syncthreads();
+        return pos;
+    }
+};
+
+// bvh 0.7.1's BVH::build for one node of >= 2 shapes (host/hikari.cpp Builder::build) over the shapes of `sg`, by a team: the
+// node's own bound (its navigator, unless the parent left it the empty box), the centre bounds and the largest axis, the six
+// buckets, the SAH candidates, and the children's shape lists in idx[!parity] — bucket by bucket, each bucket in the order the
+// shapes had (a stable counting sort), or the two halves in order when the centres coincide or one side would be empty.
+// Every thread of the team returns the same two children.
+template <class Team>
+__device__ void sah_split(Team& team, const BuildSeg& sg, const BuildIn& in, BuildSeg& l, BuildSeg& r) {
+    const uint32_t* idx_cur = in.idx[(sg.flags & SEG_IDX_B) ? 1 : 0];
+    uint32_t* idx_nxt = in.idx[(sg.flags & SEG_IDX_B) ? 0 : 1];
+    const uint32_t me = team.rank(), step = team.size();
+    // bounds of the shapes' boxes (in order) and of their centres
+    OrderedBox ab;
+    SBox cb;
+    ab.clear(); cb.clear();
+    for (uint32_t j = me; j < sg.count; j += step) {
+        const uint32_t shape = idx_cur[sg.begin + j];
+        const float4 lo = in.box_lo[shape], hi = in.box_hi[shape], c = in.center[shape];
+        ab.add(j, lo, hi);
+        cb.mn[0] = smin(cb.mn[0], c.x); cb.mn[1] = smin(cb.mn[1], c.y); cb.mn[2] = smin(cb.mn[2], c.z);
+        cb.mx[0] = smax(cb.mx[0], c.x); cb.mx[1] = smax(cb.mx[1], c.y); cb.mx[2] = smax(cb.mx[2], c.z);
+    }
+    {
+        float mins[6] = {ab.b.mn[0], ab.b.mn[1], ab.b.mn[2], cb.mn[0], cb.mn[1], cb.mn[2]};
+        float maxs[6] = {ab.b.mx[0], ab.b.mx[1], ab.b.mx[2], cb.mx[0], cb.mx[1], cb.mx[2]};
+        team.template reduce<6, 6, 6, 0>(mins, maxs, ab.z, nullptr);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) { ab.b.mn[k] = mins[k]; ab.b.mx[k] = maxs[k]; cb.mn[k] = mins[3 + k]; cb.mx[k] = maxs[3 + k]; }
+        ab.settle_zeros();
+    }
+    if (sg.t != 0u && me == 0u) {
+        const uint32_t at = sg.t - 1u + sg.leaves_before;
+        SBox own = ab.b;
+        if (sg.flags & SEG_EMPTY_BOX) own.clear();
+        store_node(in.out, at, own, at + 1u, at + 3u * sg.count - 1u);
+    }
+    const float sx = cb.mx[0] - cb.mn[0], sy = cb.mx[1] - cb.mn[1], sz = cb.mx[2] - cb.mn[2];
+    const int axis = (sx > sy && sx > sz) ? 0 : (sy > sz ? 1 : 2);       // AABB::largest_axis
+    const float split_axis_size = axis == 0 ? sx : (axis == 1 ? sy : sz);
+    const float axis_min = axis == 0 ? cb.mn[0] : (axis == 1 ? cb.mn[1] : cb.mn[2]);
+    uint32_t nl = 0u;
+    bool halves = split_axis_size < SCENE_BVH_EPSILON, boxes = true;
+    if (!halves) {
+        SBox bb[SCENE_BUCKETS];
+        uint32_t bn[SCENE_BUCKETS];
+#pragma unroll
+        for (int b = 0; b < SCENE_BUCKETS; ++b) { bb[b].clear(); bn[b] = 0u; }
+        for (uint32_t j = me; j < sg.count; j += step) {
+            const uint32_t shape = idx_cur[sg.begin + j];
+            const float4 lo = in.box_lo[shape], hi = in.box_hi[shape], c = in.center[shape];
+            const float ca = axis == 0 ? c.x : (axis == 1 ? c.y : c.z);
+            const uint32_t bucket = sah_bucket((ca - axis_min) / split_axis_size);
+            SBox b;
+            b.mn[0] = lo.x; b.mn[1] = lo.y; b.mn[2] = lo.z; b.mx[0] = hi.x; b.mx[1] = hi.y; b.mx[2] = hi.z;
+#pragma unroll
+            for (int q = 0; q < SCENE_BUCKETS; ++q)
+                if (bucket == (uint32_t)q) { bb[q].join(b); bn[q] += 1u; }
+        }
+        {
+            float mins[3 * SCENE_BUCKETS], maxs[3 * SCENE_BUCKETS];
+#pragma unroll
+            for (int b = 0; b < SCENE_BUCKETS; ++b)
+#pragma unroll
+                for (int k = 0; k < 3; ++k) { mins[3 * b + k] = bb[b].mn[k]; maxs[3 * b + k] = bb[b].mx[k]; }
+            team.template reduce<3 * SCENE_BUCKETS, 3 * SCENE_BUCKETS, 0, SCENE_BUCKETS>(mins, maxs, nullptr, bn);
+#pragma unroll
+            for (int b = 0; b < SCENE_BUCKETS; ++b)
+#pragma unroll
+                for (int k = 0; k < 3; ++k) { bb[b].mn[k] = mins[3 * b + k]; bb[b].mx[k] = maxs[3 * b + k]; }
+        }
+        // the split with the least SAH cost (every thread evaluates the same five candidates)
+        int min_bucket = 0;
+        float min_cost = __uint_as_float(0x7f800000u);
+        bool chosen = false;
+        const float parent_area = ab.b.surface_area();
+#pragma unroll
+        for (int i = 0; i < SCENE_BUCKETS - 1; ++i) {
+            SBox cl, cr;
+            cl.clear(); cr.clear();
+            uint32_t nlc = 0u, nrc = 0u;
+#pragma unroll
+            for (int b = 0; b < SCENE_BUCKETS; ++b) {
+                if (b <= i) { cl.join(bb[b]); nlc += bn[b]; } else { cr.join(bb[b]); nrc += bn[b]; }
+            }
+            const float cost = ((float)nlc * cl.surface_area() + (float)nrc * cr.surface_area()) / parent_area;
+            if (cost < min_cost) { min_bucket = i; min_cost = cost; chosen = true; }
+        }
+        uint32_t off[SCENE_BUCKETS];
+        uint32_t acc = 0u;
+#pragma unroll
+        for (int b = 0; b < SCENE_BUCKETS; ++b) {
+            off[b] = acc; acc += bn[b];
+            if (b <= min_bucket) nl += bn[b];
+        }
+        if (nl == 0u || nl == sg.count) {
+            halves = true;          // only non-finite boxes get here (host/hikari.cpp: the halves keep the build finite)
+        } else {
+            boxes = chosen;
+            for (uint32_t base = 0u; base < sg.count; base += step) {
+                const uint32_t j = base + me;
+                uint32_t shape = 0u, bucket = (uint32_t)SCENE_BUCKETS;
+                if (j < sg.count) {
+                    shape = idx_cur[sg.begin + j];
+                    const float4 c = in.center[shape];
+                    const float ca = axis == 0 ? c.x : (axis == 1 ? c.y : c.z);
+                    bucket = sah_bucket((ca - axis_min) / split_axis_size);
+                }
+                const uint32_t pos = team.ranks(bucket, off);
+                if (j < sg.count) idx_nxt[sg.begin + pos] = shape;
+            }
+        }
+    }
+    if (halves) {
+        nl = sg.count / 2u;
+        for (uint32_t j = me; j < sg.count; j += step) idx_nxt[sg.begin + j] = idx_cur[sg.begin + j];
+    }
+    const uint32_t flags = (boxes ? 0u : SEG_EMPTY_BOX) | ((sg.flags & SEG_IDX_B) ^ SEG_IDX_B);
+    l = BuildSeg{sg.begin, nl, sg.t + 1u, sg.leaves_before, flags, sg.mesh};
+    r = BuildSeg{sg.begin + nl, sg.count - nl, sg.t + 2u * nl, sg.leaves_before + nl, flags, sg.mesh};
+}
+
+// a node of one shape: its navigator (the shape's box, or the empty box its parent left it) and the leaf record
+__device__ void sah_leaf(const BuildSeg& sg, const BuildIn& in) {
+    const uint32_t at = sg.t - 1u + sg.leaves_before;
+    const uint32_t shape = in.idx[(sg.flags & SEG_IDX_B) ? 1 : 0][sg.begin];
+    SBox own, e;
+    own.clear(); e.clear();
+    if (!(sg.flags & SEG_EMPTY_BOX)) {
+        SBox b;
+        const float4 lo = in.box_lo[shape], hi = in.box_hi[shape];
+        b.mn[0] = lo.x; b.mn[1] = lo.y; b.mn[2] = lo.z; b.mx[0] = hi.x; b.mx[1] = hi.y; b.mx[2] = hi.z;
+        own.join(b);
+    }
+    store_node(in.out, at, own, at + 1u, at + 2u);
+    store_node(in.out, at + 1u, e, SCENE_LEAF | (shape - in.shape_base), at + 2u);
+    if (in.index_base) *reinterpret_cast<uint32_t*>(in.index_base + (size_t)shape * in.index_stride) = sg.t;
+}
+
+// The subtrees whose roots are in cur[0, *s_cur), level by level, one WARP per node; cur / nxt hold as many segments as the
+// subtrees have shapes.  Pre-order placement makes every node's records independent of the others'.
+__device__ void sah_levels(BuildSeg* cur, BuildSeg* nxt, const BuildIn& in, uint32_t* s_cur, uint32_t* s_next) {
+    const uint32_t tid = threadIdx.x, warp = tid >> 5, warps = blockDim.x >> 5;
+    WarpTeam team{tid & 31u};
+    for (;;) {
+        const uint32_t cnt = *s_cur;
+        if (cnt == 0u) break;
+        for (uint32_t s = warp; s < cnt; s += warps) {
+            const BuildSeg sg = cur[s];
+            if (sg.count == 1u) {
+                if (team.lane == 0u) sah_leaf(sg, in);
+                continue;
+            }
+            BuildSeg l, r;
+            sah_split(team, sg, in, l, r);
+            if (team.lane == 0u) {
+                const uint32_t slot = atomicAdd(s_next, 2u);
+                nxt[slot] = l; nxt[slot + 1u] = r;
+            }
+        }
+        __syncthreads();
+        if (tid == 0u) { *s_cur = *s_next; *s_next = 0u; }
+        BuildSeg* ts = cur; cur = nxt; nxt = ts;
+        __syncthreads();
+    }
+}
+
+// The TLAS / emissive BVH: one CTA, the whole tree.
 __global__ void __launch_bounds__(256) kc_build_flat_bvh(uint32_t n, const float4* __restrict__ box_lo, const float4* __restrict__ box_hi,
                                                          float4* center, uint32_t* idx_a, uint32_t* idx_b, BuildSeg* seg_a, BuildSeg* seg_b,
                                                          hk_node* out, uint8_t* index_base, uint32_t index_stride) {
     __shared__ uint32_t s_cur_count, s_next_count;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5, warps = blockDim.x >> 5;
-    const uint32_t lt = (1u << lane) - 1u;
+    const uint32_t tid = threadIdx.x;
     if (n == 0u) return;
     for (uint32_t i = tid; i < n; i += blockDim.x) {
         idx_a[i] = i;
-        const float4 lo = box_lo[i], hi = box_hi[i];
-        center[i] = make_float4(lo.x + (hi.x - lo.x) / 2.0f, lo.y + (hi.y - lo.y) / 2.0f, lo.z + (hi.z - lo.z) / 2.0f, 0.0f);   // AABB::center
+        center[i] = box_center(box_lo[i], box_hi[i]);
     }
     if (tid == 0u) {
         s_next_count = 0u;
@@ -240,143 +556,151 @@ __global__ void __launch_bounds__(256) kc_build_flat_bvh(uint32_t n, const float
             *reinterpret_cast<uint32_t*>(index_base) = 0u;
             s_cur_count = 0u;
         } else {
-            BuildSeg root;
-            root.begin = 0u; root.count = n; root.t = 0u; root.leaves_before = 0u;
-            for (int k = 0; k < 3; ++k) { root.lo[k] = 0.0f; root.hi[k] = 0.0f; }
-            seg_a[0] = root;
+            seg_a[0] = BuildSeg{0u, n, 0u, 0u, 0u, 0u};
             s_cur_count = 1u;
         }
     }
     __syncthreads();
-    BuildSeg* cur = seg_a; BuildSeg* nxt = seg_b;
-    uint32_t* idx_cur = idx_a; uint32_t* idx_nxt = idx_b;
+    const BuildIn in{box_lo, box_hi, center, {idx_a, idx_b}, out, 0u, index_base, index_stride};
+    sah_levels(seg_a, seg_b, in, &s_cur_count, &s_next_count);
+}
+
+// ------------------------------------------------------------------------------------------------ mesh assets (hk_scene_add_meshes)
+// GpuMesh::try_from (mod.rs:379-467) for a batch of meshes: k_mesh_records packs the vertices and primitives and each primitive's
+// box and centre; then the BLAS of every mesh, bvh 0.7.1's build + flatten_custom at mesh scale, in two launches that need neither a
+// grid-wide barrier nor a count read back by the host:
+//   kc_build_blas_top     one 1024-thread CTA per mesh splits every node of more than BLAS_TOP_SHAPES shapes, level by level, the
+//                         whole CTA on one node (sah_split with a CtaTeam); every smaller node goes to a work list
+//   kc_build_blas_bottom  CTAs take work-list entries by atomic counter and finish each subtree with the TLAS builder's loop
+//                         (sah_levels, one warp per node)
+constexpr uint32_t BLAS_TOP_SHAPES = 4096u;
+constexpr uint32_t BLAS_TOP_THREADS = 1024u, BLAS_BOTTOM_THREADS = 256u;
+
+__device__ __forceinline__ uint32_t mesh_of(const MeshJob* jobs, uint32_t n_jobs, uint32_t i, bool by_vertex) {
+    uint32_t lo = 0u, hi = n_jobs;        // the last job whose first element is <= i
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) / 2u;
+        if ((by_vertex ? jobs[mid].src_vertex : jobs[mid].shape_begin) <= i) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+__global__ void __launch_bounds__(128) k_mesh_records(uint32_t n_jobs, const MeshJob* __restrict__ jobs, uint32_t total_vertices,
+                                                      uint32_t total_primitives, const float* __restrict__ positions,
+                                                      const float* __restrict__ normals, const float* __restrict__ uvs,
+                                                      const uint32_t* __restrict__ indices, hk_vertex* vertices, hk_primitive* primitives,
+                                                      float4* box_lo, float4* box_hi, float4* center) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < total_vertices) {             // vertex i of the batch
+        const MeshJob& m = jobs[mesh_of(jobs, n_jobs, i, true)];
+        const uint32_t v = i - m.src_vertex;
+        hk_vertex* o = vertices + m.dst_vertex + v;
+        o->position[0] = positions[3u * (size_t)i]; o->position[1] = positions[3u * (size_t)i + 1u]; o->position[2] = positions[3u * (size_t)i + 2u];
+        o->normal[0] = normals[3u * (size_t)i]; o->normal[1] = normals[3u * (size_t)i + 1u]; o->normal[2] = normals[3u * (size_t)i + 2u];
+        o->u = uvs[2u * (size_t)i]; o->v = uvs[2u * (size_t)i + 1u];
+    }
+    if (i < total_primitives) {           // primitive i of the batch
+        const MeshJob& m = jobs[mesh_of(jobs, n_jobs, i, false)];
+        const uint32_t p = i - m.shape_begin;
+        uint32_t id[3];
+        if (m.strip) {                    // mod.rs:433-450: odd triangles swap their first two vertices
+            const uint32_t a = p, b = p + 1u, c = p + 2u;
+            const uint32_t va = m.indexed ? indices[m.src_index + a] : a, vb = m.indexed ? indices[m.src_index + b] : b;
+            id[0] = (p & 1u) ? vb : va; id[1] = (p & 1u) ? va : vb;
+            id[2] = m.indexed ? indices[m.src_index + c] : c;
+        } else {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) id[k] = m.indexed ? indices[m.src_index + 3u * p + (uint32_t)k] : 3u * p + (uint32_t)k;
+        }
+        float pos[3][3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) pos[k][c] = positions[3u * ((size_t)m.src_vertex + id[k]) + (uint32_t)c];
+        float4* o = reinterpret_cast<float4*>(primitives + m.dst_primitive + p);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) o[k] = make_float4(pos[k][0], pos[k][1], pos[k][2], __uint_as_float(id[k]));
+        float lo[3], hi[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {     // std::min(std::min(a, b), c) as GpuMesh::try_from
+            lo[c] = smin(smin(pos[0][c], pos[1][c]), pos[2][c]);
+            hi[c] = smax(smax(pos[0][c], pos[1][c]), pos[2][c]);
+        }
+        const float4 l4 = make_float4(lo[0], lo[1], lo[2], 0.0f), h4 = make_float4(hi[0], hi[1], hi[2], 0.0f);
+        box_lo[i] = l4; box_hi[i] = h4; center[i] = box_center(l4, h4);
+    }
+}
+
+struct BlasScratch {          // hk_blas_scratch_bytes
+    unsigned long long* counters;       // [0] work-list entries, [1] entries taken
+    float4 *box_lo, *box_hi, *center;   // per primitive of the batch
+    uint32_t *idx_a, *idx_b;
+    BuildSeg *seg_a, *seg_b, *work;
+};
+
+__device__ __forceinline__ BuildIn blas_in(const MeshJob& m, const BlasScratch& s, hk_node* nodes) {
+    return BuildIn{s.box_lo, s.box_hi, s.center, {s.idx_a, s.idx_b}, nodes + m.dst_node, m.shape_begin, nullptr, 0u};
+}
+
+__global__ void __launch_bounds__(BLAS_TOP_THREADS) kc_build_blas_top(const MeshJob* __restrict__ jobs, BlasScratch s, hk_node* nodes) {
+    __shared__ CtaTeamShared s_team;
+    __shared__ uint32_t s_cur_count, s_next_count;
+    const uint32_t tid = threadIdx.x;
+    const MeshJob m = jobs[blockIdx.x];
+    const BuildIn in = blas_in(m, s, nodes);
+    for (uint32_t i = tid; i < m.shapes; i += blockDim.x) s.idx_a[m.shape_begin + i] = m.shape_begin + i;
+    const BuildSeg root{m.shape_begin, m.shapes, 0u, 0u, 0u, blockIdx.x};
+    if (m.shapes <= BLAS_TOP_SHAPES) {
+        if (tid == 0u) {
+            if (m.shapes == 1u) {         // a single primitive: one leaf record without a navigator
+                SBox e; e.clear();
+                store_node(in.out, 0u, e, SCENE_LEAF | 0u, 1u);
+            } else {
+                s.work[atomicAdd(s.counters, 1ull)] = root;
+            }
+        }
+        return;
+    }
+    BuildSeg* cur = s.seg_a + m.shape_begin;
+    BuildSeg* nxt = s.seg_b + m.shape_begin;
+    if (tid == 0u) { cur[0] = root; s_cur_count = 1u; s_next_count = 0u; }
+    __syncthreads();
+    CtaTeam team{&s_team, tid, blockDim.x >> 5};
     for (;;) {
         const uint32_t cnt = s_cur_count;
         if (cnt == 0u) break;
-        for (uint32_t s = warp; s < cnt; s += warps) {
-            const BuildSeg sg = cur[s];
-            const uint32_t at = sg.t - 1u + sg.leaves_before;        // navigator record (not for the root)
-            SBox own;
-            for (int k = 0; k < 3; ++k) { own.mn[k] = sg.lo[k]; own.mx[k] = sg.hi[k]; }
-            if (sg.count == 1u) {
-                if (lane == 0u) {
-                    const uint32_t shape = idx_cur[sg.begin];
-                    SBox e; e.clear();
-                    store_node(out, at, own, at + 1u, at + 2u);
-                    store_node(out, at + 1u, e, SCENE_LEAF | shape, at + 2u);
-                    *reinterpret_cast<uint32_t*>(index_base + (size_t)shape * index_stride) = sg.t;
+        for (uint32_t k = 0; k < cnt; ++k) {
+            const BuildSeg sg = cur[k];
+            BuildSeg ch[2];
+            sah_split(team, sg, in, ch[0], ch[1]);
+            if (tid == 0u)
+                for (int c = 0; c < 2; ++c) {
+                    if (ch[c].count > BLAS_TOP_SHAPES) nxt[s_next_count++] = ch[c];
+                    else s.work[atomicAdd(s.counters, 1ull)] = ch[c];
                 }
-                continue;
-            }
-            if (sg.t != 0u && lane == 0u) store_node(out, at, own, at + 1u, at + 3u * sg.count - 1u);
-            // bounds of the shapes' boxes and of their centres
-            SBox ab, cb;
-            ab.clear(); cb.clear();
-            for (uint32_t j = lane; j < sg.count; j += 32u) {
-                const uint32_t shape = idx_cur[sg.begin + j];
-                const float4 lo = box_lo[shape], hi = box_hi[shape], c = center[shape];
-                ab.mn[0] = smin(ab.mn[0], lo.x); ab.mn[1] = smin(ab.mn[1], lo.y); ab.mn[2] = smin(ab.mn[2], lo.z);
-                ab.mx[0] = smax(ab.mx[0], hi.x); ab.mx[1] = smax(ab.mx[1], hi.y); ab.mx[2] = smax(ab.mx[2], hi.z);
-                cb.mn[0] = smin(cb.mn[0], c.x); cb.mn[1] = smin(cb.mn[1], c.y); cb.mn[2] = smin(cb.mn[2], c.z);
-                cb.mx[0] = smax(cb.mx[0], c.x); cb.mx[1] = smax(cb.mx[1], c.y); cb.mx[2] = smax(cb.mx[2], c.z);
-            }
-            warp_join(ab); warp_join(cb);
-            const float sx = cb.mx[0] - cb.mn[0], sy = cb.mx[1] - cb.mn[1], sz = cb.mx[2] - cb.mn[2];
-            const int axis = (sx > sy && sx > sz) ? 0 : (sy > sz ? 1 : 2);       // AABB::largest_axis
-            const float split_axis_size = axis == 0 ? sx : (axis == 1 ? sy : sz);
-            const float axis_min = axis == 0 ? cb.mn[0] : (axis == 1 ? cb.mn[1] : cb.mn[2]);
-            SBox l_box, r_box;
-            l_box.clear(); r_box.clear();
-            uint32_t nl;
-            if (split_axis_size < SCENE_BVH_EPSILON) {
-                // the centres coincide along every axis: halves in the order the shapes have
-                nl = sg.count / 2u;
-                for (uint32_t j = lane; j < sg.count; j += 32u) {
-                    const uint32_t shape = idx_cur[sg.begin + j];
-                    const float4 lo = box_lo[shape], hi = box_hi[shape];
-                    SBox b;
-                    b.mn[0] = lo.x; b.mn[1] = lo.y; b.mn[2] = lo.z; b.mx[0] = hi.x; b.mx[1] = hi.y; b.mx[2] = hi.z;
-                    if (j < nl) l_box.join(b); else r_box.join(b);
-                    idx_nxt[sg.begin + j] = shape;
-                }
-                warp_join(l_box); warp_join(r_box);
-            } else {
-                SBox bb[SCENE_BUCKETS];
-                uint32_t bn[SCENE_BUCKETS];
-#pragma unroll
-                for (int b = 0; b < SCENE_BUCKETS; ++b) { bb[b].clear(); bn[b] = 0u; }
-                for (uint32_t j = lane; j < sg.count; j += 32u) {
-                    const uint32_t shape = idx_cur[sg.begin + j];
-                    const float4 lo = box_lo[shape], hi = box_hi[shape], c = center[shape];
-                    const float ca = axis == 0 ? c.x : (axis == 1 ? c.y : c.z);
-                    const float rel = (ca - axis_min) / split_axis_size;
-                    const uint32_t bucket = (uint32_t)(rel * ((float)SCENE_BUCKETS - 0.01f));
-                    SBox b;
-                    b.mn[0] = lo.x; b.mn[1] = lo.y; b.mn[2] = lo.z; b.mx[0] = hi.x; b.mx[1] = hi.y; b.mx[2] = hi.z;
-#pragma unroll
-                    for (int q = 0; q < SCENE_BUCKETS; ++q)
-                        if (bucket == (uint32_t)q) { bb[q].join(b); bn[q] += 1u; }
-                }
-#pragma unroll
-                for (int b = 0; b < SCENE_BUCKETS; ++b) { warp_join(bb[b]); bn[b] = warp_sum(bn[b]); }
-                // the split with the least SAH cost (every lane evaluates the same five candidates)
-                int min_bucket = 0;
-                float min_cost = __uint_as_float(0x7f800000u);
-                const float parent_area = ab.surface_area();
-#pragma unroll
-                for (int i = 0; i < SCENE_BUCKETS - 1; ++i) {
-                    SBox cl, cr;
-                    cl.clear(); cr.clear();
-                    uint32_t nlc = 0u, nrc = 0u;
-#pragma unroll
-                    for (int b = 0; b < SCENE_BUCKETS; ++b) {
-                        if (b <= i) { cl.join(bb[b]); nlc += bn[b]; } else { cr.join(bb[b]); nrc += bn[b]; }
-                    }
-                    const float cost = ((float)nlc * cl.surface_area() + (float)nrc * cr.surface_area()) / parent_area;
-                    if (cost < min_cost) { min_bucket = i; min_cost = cost; l_box = cl; r_box = cr; }
-                }
-                // children = the buckets' shapes, bucket by bucket, each bucket in the order the shapes had: a stable counting sort
-                uint32_t off[SCENE_BUCKETS];
-                uint32_t acc = 0u;
-                nl = 0u;
-#pragma unroll
-                for (int b = 0; b < SCENE_BUCKETS; ++b) {
-                    off[b] = acc; acc += bn[b];
-                    if (b <= min_bucket) nl += bn[b];
-                }
-                for (uint32_t base = 0u; base < sg.count; base += 32u) {
-                    const uint32_t j = base + lane;
-                    const bool valid = j < sg.count;
-                    uint32_t shape = 0u, bucket = 0xFFFFFFFFu;
-                    if (valid) {
-                        shape = idx_cur[sg.begin + j];
-                        const float4 c = center[shape];
-                        const float ca = axis == 0 ? c.x : (axis == 1 ? c.y : c.z);
-                        const float rel = (ca - axis_min) / split_axis_size;
-                        bucket = (uint32_t)(rel * ((float)SCENE_BUCKETS - 0.01f));
-                    }
-#pragma unroll
-                    for (int b = 0; b < SCENE_BUCKETS; ++b) {
-                        const uint32_t mask = __ballot_sync(0xffffffffu, valid && bucket == (uint32_t)b);
-                        if (valid && bucket == (uint32_t)b) idx_nxt[sg.begin + off[b] + (uint32_t)__popc(mask & lt)] = shape;
-                        off[b] += (uint32_t)__popc(mask);
-                    }
-                }
-            }
-            if (lane == 0u) {
-                const uint32_t slot = atomicAdd(&s_next_count, 2u);
-                BuildSeg l, r;
-                l.begin = sg.begin; l.count = nl; l.t = sg.t + 1u; l.leaves_before = sg.leaves_before;
-                r.begin = sg.begin + nl; r.count = sg.count - nl; r.t = sg.t + 2u * nl; r.leaves_before = sg.leaves_before + nl;
-                for (int k = 0; k < 3; ++k) { l.lo[k] = l_box.mn[k]; l.hi[k] = l_box.mx[k]; r.lo[k] = r_box.mn[k]; r.hi[k] = r_box.mx[k]; }
-                nxt[slot] = l; nxt[slot + 1u] = r;
-            }
+            __syncthreads();
         }
-        __syncthreads();
         if (tid == 0u) { s_cur_count = s_next_count; s_next_count = 0u; }
         BuildSeg* ts = cur; cur = nxt; nxt = ts;
-        uint32_t* ti = idx_cur; idx_cur = idx_nxt; idx_nxt = ti;
         __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(BLAS_BOTTOM_THREADS) kc_build_blas_bottom(const MeshJob* __restrict__ jobs, BlasScratch s, hk_node* nodes) {
+    __shared__ uint32_t s_cur_count, s_next_count;
+    __shared__ unsigned long long s_item;
+    const uint32_t tid = threadIdx.x;
+    const unsigned long long items = s.counters[0];
+    for (;;) {
+        if (tid == 0u) s_item = atomicAdd(s.counters + 1, 1ull);
+        __syncthreads();
+        const unsigned long long item = s_item;
+        if (item >= items) break;
+        const BuildSeg root = s.work[item];
+        BuildSeg* cur = s.seg_a + root.begin;
+        if (tid == 0u) { cur[0] = root; s_cur_count = 1u; s_next_count = 0u; }
+        __syncthreads();
+        sah_levels(cur, s.seg_b + root.begin, blas_in(jobs[root.mesh], s, nodes), &s_cur_count, &s_next_count);
     }
 }
 
@@ -715,6 +1039,40 @@ void hk_launch_build_flat_bvh(uint32_t n, const float4* box_lo, const float4* bo
 }
 size_t hk_scene_bvh_scratch_bytes(uint32_t n) {
     return sizeof(float4) * (size_t)n + 2u * sizeof(uint32_t) * (size_t)n + 16u + 2u * sizeof(hkd::BuildSeg) * (size_t)n;
+}
+// scratch: counters | box_lo, box_hi, centre float4[N] | idx uint32[2][N] | segments, work list BuildSeg[3][N]   (N primitives)
+static hkd::BlasScratch blas_scratch(uint32_t n, void* scratch) {
+    hkd::BlasScratch s;
+    uint8_t* p = reinterpret_cast<uint8_t*>(scratch);
+    s.counters = reinterpret_cast<unsigned long long*>(p); p += 16u;
+    s.box_lo = reinterpret_cast<float4*>(p); p += sizeof(float4) * (size_t)n;
+    s.box_hi = reinterpret_cast<float4*>(p); p += sizeof(float4) * (size_t)n;
+    s.center = reinterpret_cast<float4*>(p); p += sizeof(float4) * (size_t)n;
+    s.idx_a = reinterpret_cast<uint32_t*>(p); p += sizeof(uint32_t) * (size_t)n;
+    s.idx_b = reinterpret_cast<uint32_t*>(p); p += sizeof(uint32_t) * (size_t)n;
+    p = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 15u) & ~(uintptr_t)15u);
+    s.seg_a = reinterpret_cast<hkd::BuildSeg*>(p); p += sizeof(hkd::BuildSeg) * (size_t)n;
+    s.seg_b = reinterpret_cast<hkd::BuildSeg*>(p); p += sizeof(hkd::BuildSeg) * (size_t)n;
+    s.work = reinterpret_cast<hkd::BuildSeg*>(p);
+    return s;
+}
+size_t hk_blas_scratch_bytes(uint32_t primitives) {
+    return 16u + 3u * sizeof(float4) * (size_t)primitives + 2u * sizeof(uint32_t) * (size_t)primitives + 16u + 3u * sizeof(hkd::BuildSeg) * (size_t)primitives;
+}
+int hk_launch_build_meshes(uint32_t n_jobs, const MeshJob* jobs, uint32_t total_vertices, uint32_t total_primitives, const float* positions,
+                           const float* normals, const float* uvs, const uint32_t* indices, void* scratch, hk_vertex* vertices,
+                           hk_primitive* primitives, hk_node* nodes, cudaStream_t st) {
+    if (n_jobs == 0u) return 0;
+    const hkd::BlasScratch s = blas_scratch(total_primitives, scratch);
+    cudaMemsetAsync(s.counters, 0, 16u, st);
+    const uint32_t threads = total_vertices > total_primitives ? total_vertices : total_primitives;
+    k_mesh_records<<<(threads + 127u) / 128u, 128, 0, st>>>(n_jobs, jobs, total_vertices, total_primitives, positions, normals, uvs, indices,
+                                                            vertices, primitives, s.box_lo, s.box_hi, s.center);
+    kc_build_blas_top<<<n_jobs, hkd::BLAS_TOP_THREADS, 0, st>>>(jobs, s, nodes);
+    // at most 2 N / BLAS_TOP_SHAPES + n_jobs subtrees from the top levels; enough CTAs to fill the device, and no more than the work
+    const uint32_t want = n_jobs + 2u * (total_primitives / hkd::BLAS_TOP_SHAPES) + 1u, bottom = want < 1056u ? want : 1056u;
+    kc_build_blas_bottom<<<bottom, hkd::BLAS_BOTTOM_THREADS, 0, st>>>(jobs, s, nodes);
+    return 3;
 }
 // scratch: rec_kids uint4[3n - 1] | wn_kids, wn_child uint4[n - 1] | rec_meta uint32[3n - 1] | six uint32[n - 1] | level uint32[n + 1]
 static hkd::WideScratch wide_scratch(uint32_t n, void* scratch) {

@@ -302,7 +302,7 @@ bool scale_within(const float a[3], const float b[3]) {
 }  // namespace
 
 // ================================================================================================= GpuMesh
-PrepareMeshError GpuMesh::try_from(const Mesh& mesh, GpuMesh* out) {  // mod.rs:379-467
+PrepareMeshError GpuMesh::try_from(const Mesh& mesh, GpuMesh* out, bool build_bvh) {  // mod.rs:379-467
     if (mesh.positions.empty()) return PrepareMeshError::MissingAttributePosition;
     if (mesh.normals.empty()) return PrepareMeshError::MissingAttributeNormal;
     if (mesh.uvs.empty()) return PrepareMeshError::MissingAttributeUV;
@@ -338,6 +338,8 @@ PrepareMeshError GpuMesh::try_from(const Mesh& mesh, GpuMesh* out) {  // mod.rs:
         return PrepareMeshError::IncompatiblePrimitiveTopology;
     }
     if (out->primitives.empty()) return PrepareMeshError::NoPrimitive;
+    out->nodes.clear();
+    if (!build_bvh) return PrepareMeshError::Ok;
     std::vector<std::array<float, 3>> mn(out->primitives.size()), mx(out->primitives.size());
     for (size_t i = 0; i < out->primitives.size(); ++i)
         for (int k = 0; k < 3; ++k) {
@@ -393,7 +395,16 @@ std::vector<hk_alias_entry> GpuMesh::build_alias_table(const float transform[16]
 }
 
 // ======================================================================================= MeshMaterialWorld
-uint32_t MeshMaterialWorld::add_mesh(const Mesh& mesh) { meshes_.push_back(mesh); return (uint32_t)meshes_.size() - 1; }
+uint32_t MeshMaterialWorld::add_mesh(const Mesh& mesh) {
+    meshes_.push_back(mesh);
+    device_mesh_.resize(meshes_.size(), false);
+    return (uint32_t)meshes_.size() - 1;
+}
+uint32_t MeshMaterialWorld::add_device_mesh(const Mesh& mesh) {
+    const uint32_t id = add_mesh(mesh);
+    device_mesh_[id] = true;
+    return id;
+}
 uint32_t MeshMaterialWorld::add_material(const StandardMaterial& m) { materials_in_.push_back(m); return (uint32_t)materials_in_.size() - 1; }
 void MeshMaterialWorld::set_material(uint32_t id, const StandardMaterial& m) { if (id < materials_in_.size()) materials_in_[id] = m; }
 uint32_t MeshMaterialWorld::add_instance(const InstanceDesc& i) { instances_in_.push_back(i); return (uint32_t)instances_in_.size() - 1; }
@@ -427,17 +438,27 @@ void MeshMaterialWorld::prepare_mesh_assets() {  // mesh.rs:106-166
     mesh_errors_.assign(meshes_.size(), PrepareMeshError::Ok);
     mesh_index_.assign(meshes_.size(), hk_mesh_index{0, 0, 0, 0});
     vertices.clear(); primitives.clear(); asset_nodes.clear();
+    device_mesh_.resize(meshes_.size(), false);
+    bool any_device = false;
+    uint32_t device_nodes = 0;          // BLAS records of the device meshes so far: they sit behind the host meshes' records
+    host_vertex_count_ = host_primitive_count_ = 0;
     for (size_t i = 0; i < meshes_.size(); ++i) {
-        PrepareMeshError e = GpuMesh::try_from(meshes_[i], &gpu_meshes_[i]);
+        const bool on_device = device_mesh_[i];
+        PrepareMeshError e = GpuMesh::try_from(meshes_[i], &gpu_meshes_[i], !on_device);
         mesh_errors_[i] = e;
         if (e != PrepareMeshError::Ok) continue;  // silently dropped (mesh.rs:128-137)
         mesh_ok_[i] = true;
         const GpuMesh& g = gpu_meshes_[i];
-        mesh_index_[i] = hk_mesh_index{(uint32_t)vertices.size(), (uint32_t)primitives.size(), (uint32_t)asset_nodes.size(),
-                                       (uint32_t)g.nodes.size()};
+        // hk_scene_add_meshes: 1 record for one primitive, 3 m - 2 for m >= 2 (bvh 0.7.1's flatten_custom)
+        const size_t m = g.primitives.size();
+        const uint32_t nodes = on_device ? (uint32_t)(m == 1 ? 1 : 3 * m - 2) : (uint32_t)g.nodes.size();
+        mesh_index_[i] = hk_mesh_index{(uint32_t)vertices.size(), (uint32_t)primitives.size(), (uint32_t)asset_nodes.size() + device_nodes, nodes};
+        if (!on_device && !any_device) { host_vertex_count_ += (uint32_t)g.vertices.size(); host_primitive_count_ += (uint32_t)m; }
+        any_device = any_device || on_device;
         vertices.insert(vertices.end(), g.vertices.begin(), g.vertices.end());
         primitives.insert(primitives.end(), g.primitives.begin(), g.primitives.end());
-        asset_nodes.insert(asset_nodes.end(), g.nodes.begin(), g.nodes.end());
+        if (on_device) device_nodes += nodes;
+        else asset_nodes.insert(asset_nodes.end(), g.nodes.begin(), g.nodes.end());
     }
 }
 
@@ -603,8 +624,10 @@ void MeshMaterialWorld::prepare() { prepare_mesh_assets(); prepare_material_asse
 hk_scene_desc MeshMaterialWorld::scene_desc() const {
     hk_scene_desc d;
     memset(&d, 0, sizeof(d));
-    d.vertices = vertices.data(); d.vertex_count = (uint32_t)vertices.size();
-    d.primitives = primitives.data(); d.primitive_count = (uint32_t)primitives.size();
+    // the host meshes only: the device meshes' records are built on the device (a world without them has every mesh here)
+    const bool device = std::find(device_mesh_.begin(), device_mesh_.end(), true) != device_mesh_.end();
+    d.vertices = vertices.data(); d.vertex_count = device ? host_vertex_count_ : (uint32_t)vertices.size();
+    d.primitives = primitives.data(); d.primitive_count = device ? host_primitive_count_ : (uint32_t)primitives.size();
     d.asset_nodes = asset_nodes.data(); d.asset_node_count = (uint32_t)asset_nodes.size();
     d.alias_table = alias_table.data(); d.alias_count = (uint32_t)alias_table.size();
     d.instances = instances.data(); d.instance_count = (uint32_t)instances.size();

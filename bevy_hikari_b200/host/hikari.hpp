@@ -100,7 +100,8 @@ struct GpuMesh {                              // mod.rs:310-315
     std::vector<hk_vertex> vertices;
     std::vector<hk_primitive> primitives;     // already "compact" (mod.rs:121-145)
     std::vector<hk_node> nodes;
-    static PrepareMeshError try_from(const Mesh& mesh, GpuMesh* out);                      // mod.rs:379-467
+    // mod.rs:379-467; build_bvh = false: records only, for a mesh whose BLAS is built on the device (hk_scene_add_meshes)
+    static PrepareMeshError try_from(const Mesh& mesh, GpuMesh* out, bool build_bvh = true);
     std::vector<float> transformed_primitive_areas(const float transform[16]) const;       // mod.rs:318-328
     std::vector<hk_alias_entry> build_alias_table(const float transform[16]) const;        // mod.rs:330-376
 };
@@ -134,6 +135,13 @@ class MeshMaterialWorld {
 public:
     HikariUniversalSettings universal_settings;
     uint32_t add_mesh(const Mesh& mesh);                   // Assets<Mesh>::add + extract (mesh.rs:77-104); id = asset order
+    // A mesh whose BLAS lives on the device (HikariScene::add_meshes builds it there): prepare_mesh_assets keeps its vertices and
+    // primitives on the host (the alias tables of emissive instances need the primitives' areas) and gives it the hk_mesh_index the
+    // device gives it, but builds no BVH.  Device meshes come after every host mesh of the world, and are added to the scene in
+    // world order after the world's upload; scene_desc() holds the host meshes only, so that upload never carries their records.
+    uint32_t add_device_mesh(const Mesh& mesh);
+    const Mesh& mesh(uint32_t id) const { return meshes_[id]; }
+    bool is_device_mesh(uint32_t id) const { return id < device_mesh_.size() && device_mesh_[id]; }
     uint32_t add_material(const StandardMaterial& m);      // id = rank in the BTreeMap (material.rs:162-165)
     void set_material(uint32_t id, const StandardMaterial& m);   // Assets<StandardMaterial> modified -> prepare_material_assets + prepare_instances
     uint32_t add_texture(const hk_texture_desc& t, const uint8_t* pixels);
@@ -174,6 +182,8 @@ public:
 
 private:
     std::vector<Mesh> meshes_;
+    std::vector<bool> device_mesh_;                         // per mesh: its BLAS is built on the device
+    uint32_t host_vertex_count_ = 0, host_primitive_count_ = 0;   // the records of the host meshes (scene_desc)
     std::vector<GpuMesh> gpu_meshes_;
     std::vector<bool> mesh_ok_;
     std::vector<PrepareMeshError> mesh_errors_;
@@ -242,6 +252,9 @@ public:
     // Animated instances through the device-side rebuild (hk_scene_update_transforms) whenever only transforms changed since the
     // last prepare_instances; otherwise world.prepare_instances() + hk_scene_update_instances.  *used_device_path says which.
     int update_transforms(MeshMaterialWorld& world, bool* used_device_path = nullptr);
+    // hk_scene_add_meshes for the world's device meshes `ids` (in world order, each once): their records and BLAS are built on the
+    // device; out (may be NULL) receives their hk_mesh_index, which prepare_mesh_assets gives them as well
+    int add_meshes(const MeshMaterialWorld& world, const uint32_t* ids, uint32_t n, hk_mesh_index* out);
     hk_shared_scene* handle() const { return scene_; }      // NULL for a camera's private scene
     std::string last_error() const;
 
@@ -272,6 +285,8 @@ public:
     // Animated instances through the device-side rebuild (hk_scene_update_transforms) whenever only transforms changed since the
     // last prepare_instances; otherwise world.prepare_instances() + hk_scene_update_instances.  *used_device_path says which.
     int update_transforms(MeshMaterialWorld& world, bool* used_device_path = nullptr);
+    // HikariScene::add_meshes on the camera's private scene
+    int add_meshes(const MeshMaterialWorld& world, const uint32_t* ids, uint32_t n, hk_mesh_index* out);
     // Render `scene` (a HikariScene after create()) instead of the camera's private scene; the reservoirs are kept.  From then on the
     // plugin's own upload / update calls are refused: the scene is updated once per frame through `scene` for every camera.
     int attach_scene(HikariScene& scene);

@@ -49,8 +49,8 @@ hikari_world* hikari_world_create(void) { return reinterpret_cast<hikari_world*>
 void hikari_world_destroy(hikari_world* w) { delete reinterpret_cast<MeshMaterialWorld*>(w); }
 static MeshMaterialWorld* W(hikari_world* w) { return reinterpret_cast<MeshMaterialWorld*>(w); }
 
-uint32_t hikari_world_add_mesh(hikari_world* w, const float* positions, const float* normals, const float* uvs,
-                               uint32_t vertex_count, const uint32_t* indices, uint32_t index_count, uint32_t topology) {
+static Mesh make_mesh(const float* positions, const float* normals, const float* uvs, uint32_t vertex_count, const uint32_t* indices,
+                      uint32_t index_count, uint32_t topology) {
     Mesh m;
     if (positions) { m.positions.resize(vertex_count); memcpy(m.positions.data(), positions, 12u * vertex_count); }
     if (normals) { m.normals.resize(vertex_count); memcpy(m.normals.data(), normals, 12u * vertex_count); }
@@ -59,7 +59,15 @@ uint32_t hikari_world_add_mesh(hikari_world* w, const float* positions, const fl
     if (indices) m.indices.assign(indices, indices + index_count);
     m.topology = topology == 0 ? PrimitiveTopology::TriangleList
                                : (topology == 1 ? PrimitiveTopology::TriangleStrip : PrimitiveTopology::Other);
-    return W(w)->add_mesh(m);
+    return m;
+}
+uint32_t hikari_world_add_mesh(hikari_world* w, const float* positions, const float* normals, const float* uvs,
+                               uint32_t vertex_count, const uint32_t* indices, uint32_t index_count, uint32_t topology) {
+    return W(w)->add_mesh(make_mesh(positions, normals, uvs, vertex_count, indices, index_count, topology));
+}
+uint32_t hikari_world_add_device_mesh(hikari_world* w, const float* positions, const float* normals, const float* uvs,
+                                      uint32_t vertex_count, const uint32_t* indices, uint32_t index_count, uint32_t topology) {
+    return W(w)->add_device_mesh(make_mesh(positions, normals, uvs, vertex_count, indices, index_count, topology));
 }
 static StandardMaterial to_standard_material(const hk_material* m);
 void hikari_world_set_material(hikari_world* w, uint32_t id, const hk_material* m) { W(w)->set_material(id, to_standard_material(m)); }

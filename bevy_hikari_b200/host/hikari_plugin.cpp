@@ -1,6 +1,8 @@
 // hikari_plugin.cpp — the part of the host mirror that CALLS the C ABI: the three render-graph nodes and HikariPlugin.
 // Linked into libhikari_b200.so; everything else of the mirror (scene preparation, settings, frame uniforms) is in
 // libhikari_host.so, which has no CUDA dependency at all (the CPU reference arm of bench.py loads only that one).
+#include <algorithm>
+
 #include "hikari.hpp"
 
 namespace hikari {
@@ -43,6 +45,26 @@ int HikariScene::update_transforms(MeshMaterialWorld& world, bool* used_device_p
     world.prepare_instances();
     return update_instances(world);
 }
+int HikariScene::add_meshes(const MeshMaterialWorld& world, const uint32_t* ids, uint32_t n, hk_mesh_index* out) {
+    if (!scene_ && !ctx_) return HK_ERR_NOT_READY;
+    std::vector<hk_mesh_source> src(n);
+    for (uint32_t i = 0; i < n; ++i) {
+        const Mesh& m = world.mesh(ids[i]);
+        hk_mesh_source& s = src[i];
+        s.positions = m.positions.empty() ? nullptr : m.positions[0].data(); s.position_count = (uint32_t)m.positions.size();
+        s.normals = m.normals.empty() ? nullptr : m.normals[0].data(); s.normal_count = (uint32_t)m.normals.size();
+        s.uvs = m.uvs.empty() ? nullptr : m.uvs[0].data(); s.uv_count = (uint32_t)m.uvs.size();
+        static const uint32_t none = 0;
+        s.indices = m.has_indices ? (m.indices.empty() ? &none : m.indices.data()) : nullptr;
+        s.index_count = (uint32_t)m.indices.size();
+        s.topology = m.topology == PrimitiveTopology::TriangleList ? HK_TOPOLOGY_TRIANGLE_LIST
+                     : (m.topology == PrimitiveTopology::TriangleStrip ? HK_TOPOLOGY_TRIANGLE_STRIP : 0xFFFFFFFFu);
+    }
+    std::vector<hk_mesh_index> got(n);
+    const int rc = scene_ ? hk_shared_scene_add_meshes(scene_, src.data(), n, got.data()) : hk_scene_add_meshes(ctx_, src.data(), n, got.data());
+    if (rc == HK_OK && out) std::copy(got.begin(), got.end(), out);
+    return rc;
+}
 std::string HikariScene::last_error() const {
     if (scene_) return hk_shared_scene_last_error(scene_);
     return ctx_ ? hk_last_error(ctx_) : "";
@@ -66,6 +88,9 @@ int HikariPlugin::build_tile(int cuda_device, uint32_t width, uint32_t height, u
 int HikariPlugin::upload_scene(const MeshMaterialWorld& world) { return scene_.upload(world); }
 int HikariPlugin::update_instances(const MeshMaterialWorld& world) { return scene_.update_instances(world); }
 int HikariPlugin::update_transforms(MeshMaterialWorld& world, bool* used_device_path) { return scene_.update_transforms(world, used_device_path); }
+int HikariPlugin::add_meshes(const MeshMaterialWorld& world, const uint32_t* ids, uint32_t n, hk_mesh_index* out) {
+    return scene_.add_meshes(world, ids, n, out);
+}
 int HikariPlugin::attach_scene(HikariScene& scene) {
     if (!ctx_) return HK_ERR_NOT_READY;
     if (!scene.handle()) return HK_ERR_INVALID_ARGUMENT;     // a camera's private scene is not shared

@@ -38,6 +38,9 @@ int hikari_plugin_run_frame(hikari_plugin* p, const hikari_settings* s, const hk
     v.view = *view; v.previous_view = *previous_view; v.lights = *lights;
     return P(p)->run_frame(to_cpp(s), v);
 }
+int hikari_plugin_add_meshes(hikari_plugin* p, hikari_world* w, const uint32_t* mesh_ids, uint32_t n, hk_mesh_index* out) {
+    return P(p)->add_meshes(*W(w), mesh_ids, n, out);
+}
 hk_context* hikari_plugin_context(hikari_plugin* p) { return P(p)->context(); }
 uint64_t hikari_plugin_frame_counter(hikari_plugin* p) { return P(p)->counter.value; }
 void hikari_plugin_set_frame_counter(hikari_plugin* p, uint64_t v) { P(p)->counter.value = (size_t)v; }
@@ -55,6 +58,9 @@ int hikari_shared_scene_update_transforms(hikari_shared_scene* s, hikari_world* 
     int rc = S(s)->update_transforms(*W(w), &used);
     if (used_device_path) *used_device_path = used ? 1 : 0;
     return rc;
+}
+int hikari_shared_scene_add_meshes(hikari_shared_scene* s, hikari_world* w, const uint32_t* mesh_ids, uint32_t n, hk_mesh_index* out) {
+    return S(s)->add_meshes(*W(w), mesh_ids, n, out);
 }
 hk_shared_scene* hikari_shared_scene_handle(hikari_shared_scene* s) { return S(s)->handle(); }
 int hikari_plugin_attach_scene(hikari_plugin* p, hikari_shared_scene* s) { return s ? P(p)->attach_scene(*S(s)) : P(p)->detach_scene(); }

@@ -120,6 +120,15 @@ OUT_GBUFFER_INSTANCE_MATERIAL, OUT_GBUFFER_VELOCITY_UV = 19, 20
 OUT_RESERVOIR_0 = 32
 SCENE_INSTANCES, SCENE_INSTANCE_NODES, SCENE_EMISSIVES, SCENE_EMISSIVE_NODES, SCENE_PREVIOUS_MODELS, SCENE_INSTANCE_MOVED = range(6)   # hk_scene_readback
 SCENE_WIDE_TLAS, SCENE_WIDE_INSTANCE_RANK = 6, 7
+SCENE_VERTICES, SCENE_PRIMITIVES, SCENE_ASSET_NODES = 8, 9, 10
+TOPOLOGY_TRIANGLE_LIST, TOPOLOGY_TRIANGLE_STRIP = 0, 1
+
+
+class MeshSource(C.Structure):
+    """hk_mesh_source (include/hikari_b200.h): one mesh for hk_scene_add_meshes."""
+    _fields_ = [("positions", C.c_void_p), ("position_count", C.c_uint32), ("normals", C.c_void_p), ("normal_count", C.c_uint32),
+                ("uvs", C.c_void_p), ("uv_count", C.c_uint32), ("indices", C.c_void_p), ("index_count", C.c_uint32),
+                ("topology", C.c_uint32)]
 WIDE_NODE = np.dtype([("lo_x", f4, 4), ("lo_y", f4, 4), ("lo_z", f4, 4), ("hi_x", f4, 4), ("hi_y", f4, 4), ("hi_z", f4, 4),
                       ("child", u4, 4), ("pad", u4, 4)])      # hk_wide_node (csrc/hk_wide.cuh), 128 bytes
 assert WIDE_NODE.itemsize == 128

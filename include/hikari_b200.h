@@ -212,6 +212,32 @@ int hk_scene_update_instances(hk_context* ctx, const hk_scene_desc* scene);
  * call never waits for the device, except for its pinned staging slot when the host is two calls ahead of the copies. */
 int hk_scene_update_transforms(hk_context* ctx, const float* models, const float* previous_models, const float* mesh_aabbs,
                                uint32_t instance_count);
+/* Meshes added to a live scene, built ON THE DEVICE (SURVEY 8(f) rank 2; the reference runs GpuMesh::try_from on the CPU for every
+ * new mesh in prepare_mesh_assets, src/mesh_material/mesh.rs:106-166, and its SAH build can stall a frame).  Each hk_mesh_source
+ * carries what try_from reads (mod.rs:379-467): positions, normals and uvs, each with its count (the vertex count is the smallest
+ * of the three, the `multizip` rule), an optional index list (NULL = non-indexed: 0, 1, 2, ...) and the topology.  The meshes are
+ * appended after those already in the scene, in the order given; out[i] receives mesh i's hk_mesh_index, the record
+ * prepare_mesh_assets makes for a mesh that sits last in its world (node_count = 1 for one primitive, 3 m - 2 for m >= 2), ready for
+ * the instances of a later hk_scene_update_instances.  Kernels on the scene's stream pack the vertex and primitive records and
+ * build every mesh's BLAS, bvh 0.7.1's bucketed SAH build + flatten_custom, record for record what host/hikari.cpp builds.  The
+ * call does not wait for the device: the arrays are staged through the scene's two pinned slots (as hk_scene_update_transforms
+ * stages its own) and are the caller's again on return.  It waits only for the copy made from the same slot two calls before, and
+ * when a batch is larger than that slot: the slot is then replaced inside the call (cudaFreeHost + cudaMallocHost, which can wait
+ * for the device and take milliseconds for large batches), and keeps that size for the scene's lifetime; buffers that grow are replaced after the frames in
+ * flight that read them.  Refused on the host before anything is launched, with the scene unchanged (HK_ERR_INVALID_ARGUMENT and
+ * the PrepareMeshError of mod.rs:301-308 or the reason in hk_last_error): a missing attribute, a list whose length is not a
+ * multiple of 3, an unknown topology, no primitive, an index at or beyond the vertex count, counts that do not fit the leaf flag
+ * (0x80000000) or 32-bit record offsets.  Meshes built on the device have no 4-wide tree: a scene whose instances use one walks the
+ * reference's arrays for every ray (HK_TUNE_WIDE_TRAVERSAL; the images are the same, hk_get_stats reports it). */
+enum { HK_TOPOLOGY_TRIANGLE_LIST = 0, HK_TOPOLOGY_TRIANGLE_STRIP = 1 };
+typedef struct hk_mesh_source {
+    const float* positions;    uint32_t position_count;   /* 3 floats each: ATTRIBUTE_POSITION */
+    const float* normals;      uint32_t normal_count;     /* 3 floats each: ATTRIBUTE_NORMAL */
+    const float* uvs;          uint32_t uv_count;         /* 2 floats each: ATTRIBUTE_UV_0 */
+    const uint32_t* indices;   uint32_t index_count;      /* NULL: non-indexed */
+    uint32_t topology;                                    /* HK_TOPOLOGY_* */
+} hk_mesh_source;
+int hk_scene_add_meshes(hk_context* ctx, const hk_mesh_source* meshes, uint32_t mesh_count, hk_mesh_index* out);
 /* Shared scenes: several cameras render ONE scene, uploaded and animated once per frame.  The reference keeps one set of scene
  * buffers for the whole render world (MeshMaterialBindGroup, src/mesh_material/mod.rs:677-681) that every camera's LightNode binds
  * (src/light.rs:641-642); only reservoirs and textures are per camera (ReservoirCache, src/light.rs:69,307-383).  Split screen, a
@@ -246,13 +272,15 @@ int hk_shared_scene_upload(hk_shared_scene* s, const hk_scene_desc* scene);
 int hk_shared_scene_update_instances(hk_shared_scene* s, const hk_scene_desc* scene);
 int hk_shared_scene_update_transforms(hk_shared_scene* s, const float* models, const float* previous_models,
                                       const float* mesh_aabbs, uint32_t instance_count);
+int hk_shared_scene_add_meshes(hk_shared_scene* s, const hk_mesh_source* meshes, uint32_t mesh_count, hk_mesh_index* out);
 const char* hk_shared_scene_last_error(hk_shared_scene* s);
 int hk_context_attach_scene(hk_context* ctx, hk_shared_scene* s);   /* NULL detaches; frees a private scene */
 /* Test / debugging aid: the per-frame scene buffers as they are on the device, in the layouts of hk_layout.h. */
 enum { HK_SCENE_INSTANCES = 0, HK_SCENE_INSTANCE_NODES = 1, HK_SCENE_EMISSIVES = 2, HK_SCENE_EMISSIVE_NODES = 3,
        HK_SCENE_PREVIOUS_MODELS = 4 /* 64 B per instance; empty when nothing moved */, HK_SCENE_INSTANCE_MOVED = 5 /* uint32 per instance */,
        HK_SCENE_WIDE_TLAS = 6 /* the 4-wide TLAS of HK_TUNE_WIDE_TRAVERSAL: 128-B nodes (csrc/hk_wide.cuh); empty when it could not be derived */,
-       HK_SCENE_WIDE_INSTANCE_RANK = 7 /* uint32 per instance: its leaf's position among the TLAS's leaf records */ };
+       HK_SCENE_WIDE_INSTANCE_RANK = 7 /* uint32 per instance: its leaf's position among the TLAS's leaf records */,
+       HK_SCENE_VERTICES = 8, HK_SCENE_PRIMITIVES = 9, HK_SCENE_ASSET_NODES = 10 /* the meshes: uploaded, then added by hk_scene_add_meshes */ };
 int hk_scene_buffer_bytes(hk_context* ctx, int which, size_t* bytes);
 int hk_scene_readback(hk_context* ctx, int which, void* host, size_t bytes);   /* bytes = hk_scene_buffer_bytes */
 int hk_set_noise(hk_context* ctx, const uint8_t* rgba8_64x64x16);   /* 16 textures of 64x64 RGBA8, lib.rs:189-219 */

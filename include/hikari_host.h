@@ -48,6 +48,11 @@ void hikari_world_destroy(hikari_world* w);
 /* topology: 0 = TriangleList, 1 = TriangleStrip, 2 = anything else.  NULL attribute => PrepareMeshError (mod.rs:301-308). */
 uint32_t hikari_world_add_mesh(hikari_world* w, const float* positions, const float* normals, const float* uvs,
                                uint32_t vertex_count, const uint32_t* indices, uint32_t index_count, uint32_t topology);
+/* The same for a mesh whose BLAS is built on the device (hikari_plugin_add_meshes / hikari_shared_scene_add_meshes): prepare keeps its
+ * vertices and primitives on the host, for the alias tables, gives it the hk_mesh_index the device gives it and builds no BVH.  Device
+ * meshes follow every host mesh, and are added to the scene in world order after the world's upload (which never carries them). */
+uint32_t hikari_world_add_device_mesh(hikari_world* w, const float* positions, const float* normals, const float* uvs,
+                                      uint32_t vertex_count, const uint32_t* indices, uint32_t index_count, uint32_t topology);
 uint32_t hikari_world_add_material(hikari_world* w, const hk_material* m);
 /* a modified StandardMaterial asset: set, then hikari_world_prepare_materials (material.rs:139-203) and
  * hikari_world_prepare_instances (emissive list / alias tables depend on the materials), then hikari_plugin_update_instances */
@@ -106,6 +111,8 @@ int hikari_plugin_update_instances(hikari_plugin* p, hikari_world* w);   /* hk_s
 /* animated instances, device-side: hk_scene_update_transforms when hikari_world_prepare_instance_transforms allows it, else
  * prepare_instances + hk_scene_update_instances; *used_device_path (may be NULL) says which */
 int hikari_plugin_update_transforms(hikari_plugin* p, hikari_world* w, int* used_device_path);
+/* hk_scene_add_meshes for the world's device meshes `mesh_ids`; out (may be NULL) receives their hk_mesh_index */
+int hikari_plugin_add_meshes(hikari_plugin* p, hikari_world* w, const uint32_t* mesh_ids, uint32_t n, hk_mesh_index* out);
 int hikari_plugin_run_frame(hikari_plugin* p, const hikari_settings* s, const hk_view* view,
                             const hk_previous_view* previous_view, const hk_lights* lights);
 hk_context* hikari_plugin_context(hikari_plugin* p);
@@ -125,6 +132,7 @@ int hikari_shared_scene_build(hikari_shared_scene* s, int cuda_device, void* cud
 int hikari_shared_scene_upload(hikari_shared_scene* s, hikari_world* w);
 int hikari_shared_scene_update_instances(hikari_shared_scene* s, hikari_world* w);
 int hikari_shared_scene_update_transforms(hikari_shared_scene* s, hikari_world* w, int* used_device_path);
+int hikari_shared_scene_add_meshes(hikari_shared_scene* s, hikari_world* w, const uint32_t* mesh_ids, uint32_t n, hk_mesh_index* out);
 hk_shared_scene* hikari_shared_scene_handle(hikari_shared_scene* s);
 /* the camera renders `s` from its next frame on, keeping its reservoirs (hk_context_attach_scene); its own upload / update calls
  * are refused while it does.  s = NULL: back to a private scene, HK_ERR_NOT_READY until hikari_plugin_upload_scene. */
