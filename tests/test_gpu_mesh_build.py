@@ -12,7 +12,7 @@ import pytest
 
 from bevy_hikari_b200 import layout as L
 from bevy_hikari_b200 import plugin, scenes
-from tests.conftest import Bench
+from tests.conftest import EMULATED, Bench
 
 pytestmark = pytest.mark.gpu
 
@@ -92,6 +92,12 @@ def soup(tris, seed, spread=10.0):
     return (pos, nrm, uv, None)
 
 
+# The two meshes above BLAS_TOP_SHAPES (4096), whose top levels a whole CTA splits: 5000 and 45 000 triangles on the device, just
+# over 4096 on the emulated kernels, whose fibers take about 5 ms per primitive (tests/test_mesh_build_edges_emulated.py holds the
+# CTA-level edges at those sizes)
+LARGE_SOUP, LARGE_GRID = (4100, 46) if EMULATED else (5000, 150)
+
+
 def edge_meshes():
     one = (np.float32([[0, 0, 0], [1, 0, 0], [0, 1, 0]]), np.float32([[0, 0, 1]] * 3), np.float32([[0, 0]] * 3), np.uint32([0, 1, 2]))
     two = (np.float32([[0, 0, 0], [1, 0, 0], [0, 1, 0], [1, 1, 0]]), np.float32([[0, 0, 1]] * 4), np.float32([[0, 0]] * 4),
@@ -108,7 +114,7 @@ def edge_meshes():
     uneven = (soup(50, 3)[0], soup(50, 3)[1][:120], soup(50, 3)[2][:100], np.arange(99, dtype=np.uint32))   # multizip: 100 vertices
     return {"one": one, "two": two, "coincident": coincident, "flat_signed_zeros": quad_grid(40), "flat_z1": quad_grid(9, z=1.0),
             "strip_even": strip_even, "strip_odd": strip_odd, "nonfinite": tuple(nonfinite), "uneven_attributes": uneven,
-            "soup_5000": soup(5000, 4), "flat_large": quad_grid(150)}
+            "soup_5000": soup(LARGE_SOUP, 4), "flat_large": quad_grid(LARGE_GRID)}
 
 
 def fresh_device(width=16, height=16):

@@ -2,7 +2,9 @@
 tests/test_scene_update_edges_emulated.py does for the device scene rebuild), so that what hk_scene_add_meshes COMPUTES — the vertex
 and primitive records and every mesh's BLAS, top levels split by a whole CTA and subtrees finished from the work list — is checked on
 any machine, in both thread orders of the emulation.  Rendering frames on the emulation is slow, so the frame comparisons and all but
-one refusal run on the device only, with the million-triangle mesh and the town and house meshes."""
+one refusal run on the device only, with the million-triangle mesh and the town and house meshes.  The meshes above 4096 primitives
+(soup_5000, flat_large) have just over 4096 here (tests/test_gpu_mesh_build.py LARGE_SOUP / LARGE_GRID): both passes take 3.5 min on
+8 cores, against 19.5 min with the device's 5000 and 45 000 triangles."""
 import os
 import shutil
 import subprocess

@@ -74,3 +74,32 @@ def test_integer_feeding_arithmetic_is_never_contracted_or_approximated(tmp_path
     assert not approx, f"{name}: approximate division / square root in the tolerance build: {approx[:4]}"
     fma = lambda text: len(re.findall(r"^\s*fma\.rn\.f32\s", text, re.M))
     assert fma(fast) == fma(exact), f"{name}: {fma(fast)} FMAs with the tolerance flags, {fma(exact)} with the exact ones"
+
+
+# hk_scene_add_meshes and the TLAS build restate bvh 0.7.1 bit for bit against the host mirror: the SAH costs, the bucket of a centre
+# and AABB::center (box_center) must round exactly as the host's f32 does, so kernels_scene.cu is compiled with the exact flags
+SCENE_BUILDERS = ["kc_build_flat_bvh", "kc_build_blas_top", "kc_build_blas_bottom", "k_mesh_records"]
+
+
+def test_scene_builders_are_never_contracted_or_approximated(tmp_path):
+    assert "csrc/kernels_scene.cu" not in product_build.FAST_TUS, "kernels_scene.cu must not be a tolerance unit"
+    if not os.path.exists(product_build.NVCC):
+        pytest.skip("no nvcc")
+    out = tmp_path / "kernels_scene.ptx"
+    flags = [f for f in product_build.probe_flags("exact") if f != "-lineinfo"]      # build.py's flags for a unit outside FAST_TUS
+    src = os.path.join(os.path.dirname(product_build.__file__), "csrc", "kernels_scene.cu")
+    r = subprocess.run([product_build.NVCC] + flags + ["-ptx", src, "-o", str(out)], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    text = out.read_text()
+    assert not re.search(r"^\s*call", text, re.M), "a device function is called, not inlined: its body must be checked too"
+    for name in SCENE_BUILDERS:
+        m = re.search(r"^\.visible \.entry _ZN3hkd\d+%s[^\n]*\n(.*?)^\}" % name, text, re.M | re.S)
+        assert m, f"{name}: no entry in the PTX"
+        body = m.group(1)
+        assert re.search(r"^\s*(?:mul|add|sub|div)\.rn\.f32\s", body, re.M), f"{name}: no f32 arithmetic found"
+        fma = re.findall(r"^\s*fma\.\S+\s.*$", body, re.M)
+        assert not fma, f"{name}: contracted into FMAs: {fma[:4]}"
+        plain = re.findall(r"^\s*(?:mul|add|sub)\.f32\s.*$", body, re.M)
+        assert not plain, f"{name}: f32 arithmetic without .rn: {plain[:4]}"
+        approx = re.findall(r"^\s*(?:div\.(?:approx|full)|sqrt\.approx|rsqrt|rcp\.approx)\S*\s.*$", body, re.M)
+        assert not approx, f"{name}: approximate division / square root: {approx[:4]}"
