@@ -926,6 +926,9 @@ __device__ __forceinline__ bool previous_pixel(const KParams& P, vec2 previous_u
     bool inside = inclusive ? (ax <= 0.5f && ay <= 0.5f) : (ax < 0.5f && ay < 0.5f);
     if (!inside) return false;
     int px = f32_to_i32(mul_rn(previous_uv.x, (float)P.band.RW)), py = f32_to_i32(mul_rn(previous_uv.y, (float)P.band.RH));
+    // the reference indexes the buffer with coords.x + size.x * coords.y: a uv of exactly 1.0 in x (which the inclusive test of the
+    // scatter admits) is column 0 of the next row, not a pixel outside the frame
+    if (px == P.band.RW) { px = 0; py += 1; }
     if (!render_allocated(P, px, py)) return false;
     pidx = render_index(P.band, px, py);
     return true;

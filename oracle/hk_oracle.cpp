@@ -858,8 +858,11 @@ struct ScatterLog {
     explicit ScatterLog(int h) : rows(h) {}
     void push(int y, int32_t index, const hk_packed_reservoir& v) { rows[y].push_back({index, v}); }
     void apply(std::vector<hk_packed_reservoir>& buf) {
+        // a previous uv of 1.0 in y, or in x on the last row, indexes past the buffer: WGSL's robust buffer access may discard the
+        // store, as the kernels do
         for (auto& row : rows)
-            for (auto& w : row) buf[w.index] = w.value;
+            for (auto& w : row)
+                if (w.index >= 0 && (size_t)w.index < buf.size()) buf[w.index] = w.value;
     }
 };
 
@@ -2272,8 +2275,8 @@ void hko_spatial_digest(uint32_t count, float range, int w, int h, uint32_t fram
 //   [0] the light passes' G-buffer texel, Deferred::jittered_coords of coords_to_uv,
 //   [1] the denoise passes' texel, Deferred::nearest of jittered_uv(uv, 0.5),
 //   [2] load_previous's pixel of jittered_uv(uv, 0.25) - velocity, with the all(< 0.5) and the all(<= 0.5) test (scatter), for
-//       velocity 0 and for the velocity math_probe.cu draws: the index, or ~0 outside.  A uv of exactly 1 passes the inclusive test
-//       with a pixel one past the row, which the device rejects: it counts as outside here too,
+//       velocity 0 and for the velocity math_probe.cu draws: the index, or ~0 outside.  The index is the reference's
+//       coords.x + size.x * coords.y: a uv of exactly 1 in x is column 0 of the next row, one past the buffer counts as outside,
 //   [3] for both tables, pass_spatial_reuse's neighbour pixels (spatial_neighbour), the texel of each one inside the frame and of each
 //       of its depth-march taps (spatial_tap_uv).
 void hko_deferred_digest(int w, int h, float ratio, uint32_t frame, uint32_t* out) {
@@ -2307,8 +2310,8 @@ void hko_deferred_digest(int w, int h, float ratio, uint32_t frame, uint32_t* ou
             for (int inclusive = 0; inclusive < 2; ++inclusive) {
                 uint32_t index = 0xFFFFFFFFu;
                 if (inclusive ? uv_inside_eq(previous_uv) : uv_inside(previous_uv)) {
-                    const bool in_frame = f32_to_i32(previous_uv.x * (float)size.x) < size.x && f32_to_i32(previous_uv.y * (float)size.y) < size.y;
-                    if (in_frame) index = (uint32_t)uv_to_index(previous_uv, size);
+                    const int32_t i = uv_to_index(previous_uv, size);
+                    if (i < size.x * size.y) index = (uint32_t)i;
                 }
                 d[2] = fnv(d[2], index);
             }

@@ -161,6 +161,29 @@ def test_moving_camera_bit_exact(scene, config, size):
     assert moved > 1000
 
 
+def test_scatter_at_previous_uv_one_lands_in_the_next_row():
+    """light.wgsl stores a reprojected write at coords.x + size.x * coords.y, and the scatter's test admits a previous uv of exactly
+    1.0: in x that is column 0 of the next row (seen on city 3840x2160 under a moving camera).  Right-edge pixels get the velocity
+    that puts their previous uv at 1.0, column-0 pixels one that takes theirs out of the frame, so the wrapped write is their only one.
+    The last row's write indexes past the buffer and is discarded on both sides."""
+    W, H = 24, 16
+    b = Bench("city", W, H, config="city_4k")              # the ground reaches both side edges
+    dev, orc = b.device(), b.oracle()
+    edge_uv = (np.float32(W - 1) + np.float32(0.5)) / np.float32(W)        # coords_to_uv of the last column
+    for f in (1, 2):
+        inp = b.inputs(f)
+        dev.prepass(inp); orc.prepass(inp)
+        vel = orc.readback(L.OUT_GBUFFER_VELOCITY_UV).copy()
+        vel[:, W - 1, 0] = edge_uv - np.float32(1.0)           # uv.x - velocity.x == 1.0 exactly
+        vel[:, 0, 0] = np.float32(0.5)                         # previous uv.x < 0: no write of its own
+        dev.upload_state(L.OUT_GBUFFER_VELOCITY_UV, vel); orc.upload_state(L.OUT_GBUFFER_VELOCITY_UV, vel)
+        for p in (0, 1, 2, 4):
+            orc.run_pass(inp, p); dev.run_pass(inp, p)
+        for k in [L.OUT_RESERVOIR_0 + i for i in range(10)]:
+            assert mismatch(dev.readback(k), orc.readback(k)) == 0, (f, k)
+    assert (orc.readback(L.OUT_GBUFFER_POSITION)[:H - 1, W - 1, 3] > 0).sum() >= 8      # surfaces at the right edge write
+
+
 def test_nodes_one_by_one_equal_render_frame():
     """hk_prepass_run + hk_light_run + hk_post_process_run (unfused tone mapping) == hk_render_frame."""
     b = Bench("cornell", 80, 48, config="cornell_1080p")
