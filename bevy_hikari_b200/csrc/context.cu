@@ -469,10 +469,6 @@ int hk_context_create_tile(hk_context** out, int cuda_device, uint32_t width, ui
     if (const char* e = getenv("HK_TUNE_TILED_DENOISE")) c->tiled_denoise = atoi(e) != 0;
     c->wide_traversal = hk_tolerance_build() != 0 ? HK_WIDE_TRAVERSAL_DEFAULT : 0;      // the exact flavour keeps the reference's walk
     if (const char* e = getenv("HK_TUNE_WIDE_TRAVERSAL")) c->wide_traversal = atoi(e) & 3;
-#ifndef HK_EMU
-    // A/B: ask for the largest L1 split for kernels that use no shared memory (the light kernels keep their spills and the scene there)
-    if (const char* e = getenv("HK_TUNE_PREFER_L1")) { if (atoi(e)) cudaDeviceSetCacheConfig(cudaFuncCachePreferL1); }
-#endif
     ctx = c;
     if (cuda_stream) c->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
     else {

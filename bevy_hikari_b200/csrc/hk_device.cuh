@@ -15,35 +15,8 @@
 #include "hikari_b200.h"
 #include "hk_math.h"
 
-// Inlining policy of the large device functions (code size vs call overhead; see DESIGN.md 4: the light kernels are
-// instruction-fetch bound).  Override per function group with -DHK_INL_<GROUP>=__noinline__.
-#ifndef HK_INL_PACK
-#define HK_INL_PACK __forceinline__
-#endif
-#ifndef HK_INL_TRAVERSE
-#define HK_INL_TRAVERSE __forceinline__
-#endif
-#ifndef HK_INL_HITINFO
-#define HK_INL_HITINFO __forceinline__
-#endif
-#ifndef HK_INL_TEXTURE
-#define HK_INL_TEXTURE __forceinline__
-#endif
-#ifndef HK_SURFACE_LOOP
-#define HK_SURFACE_LOOP 0
-#endif
-#ifndef HK_INL_SURFACE
-#define HK_INL_SURFACE __forceinline__
-#endif
-#ifndef HK_INL_SHADE
-#define HK_INL_SHADE __forceinline__
-#endif
-#ifndef HK_INL_RADIANCE
-#define HK_INL_RADIANCE __forceinline__
-#endif
-#ifndef HK_INL_SELECT
-#define HK_INL_SELECT __forceinline__
-#endif
+// The large device functions below are __forceinline__: the light kernels are instruction-fetch bound, but outlining them to
+// shrink the code was measured slower (DESIGN.md 4).
 
 namespace hkd {
 using namespace hk;
@@ -191,7 +164,7 @@ struct KParams {
     // receives this context's owned pixels at their global position; nullptr = none
     uint2* frame_target;
     uint32_t frame_pitch;   // pixels
-    float inv_rw, inv_rh;   // RN(1 / RW), RN(1 / RH), computed on the host (HK_SPATIAL_FAST_DIV)
+    float inv_rw, inv_rh;   // RN(1 / RW), RN(1 / RH), computed on the host (spatial_tap_uv, hk_spatial_taps.cuh)
     int tile_images;        // 1 = tile context with the temporal upscalers enabled: render-size images are stored over the allocation
 };
 
@@ -233,7 +206,7 @@ __device__ __forceinline__ Reservoir zero_reservoir() {
 // light.wgsl:77-136 on the planar layout.
 struct PackedQuarters { uint4 q0, q1, q2, q3; };
 
-static __device__ HK_INL_PACK Reservoir unpack_reservoir(const PackedQuarters& p) {
+static __device__ __forceinline__ Reservoir unpack_reservoir(const PackedQuarters& p) {
     Reservoir r;
     vec2 t0 = unpack2x16float(p.q3.z), t1 = unpack2x16float(p.q3.w);
     r.count = t0.x; r.w = t0.y; r.w_sum = t1.x; r.w2_sum = t1.y;
@@ -251,7 +224,7 @@ static __device__ HK_INL_PACK Reservoir unpack_reservoir(const PackedQuarters& p
     r.s.visible_instance = f32_to_u32(__uint_as_float(p.q2.w));
     return r;
 }
-static __device__ HK_INL_PACK PackedQuarters pack_reservoir(const Reservoir& r) {
+static __device__ __forceinline__ PackedQuarters pack_reservoir(const Reservoir& r) {
     PackedQuarters p;
     p.q0.x = pack2x16float(r.s.radiance.x, r.s.radiance.y);
     p.q0.y = pack2x16float(r.s.radiance.z, r.s.radiance.w);
@@ -420,7 +393,7 @@ __device__ __forceinline__ void instance_ray(const hk_instance* inst, const Ray&
 // updates and both early-outs are unchanged, so hits are bit-identical to the nested walk.
 // Ending phase 1 on a warp vote (as soon as at most 1/2 .. 1/8 of the lanes are still on interior records) instead of waiting for
 // the last lane was tried and not kept: the votes and the per-lane state machine cost what the shorter waits save.
-static __device__ HK_INL_TRAVERSE Hit traverse_top(const DeviceScene& sc, const Ray& ray, float max_distance, float early_distance,
+static __device__ __forceinline__ Hit traverse_top(const DeviceScene& sc, const Ray& ray, float max_distance, float early_distance,
                                             uint32_t exclude_instance) {
     Hit hit;
     hit.u = 0.0f; hit.v = 0.0f; hit.distance = max_distance;
@@ -517,7 +490,7 @@ __device__ __forceinline__ HitInfo empty_hit_info(vec3 position, vec3 direction)
     info.normal = v3(0.0f); info.uv = v2(0.0f, 0.0f);
     return info;
 }
-static __device__ HK_INL_HITINFO HitInfo hit_info(const DeviceScene& sc, const Ray& ray, const Hit& hit) {  // light.wgsl:496-523
+static __device__ __forceinline__ HitInfo hit_info(const DeviceScene& sc, const Ray& ray, const Hit& hit) {  // light.wgsl:496-523
     HitInfo info;
     info.instance_index = hit.instance_index;
     info.material_index = U32_MAX;
@@ -582,7 +555,7 @@ __device__ __forceinline__ int wrap_coord(int i, int n, uint32_t mode) {
     int period = 2 * n; i %= period; if (i < 0) i += period;
     return (i < n) ? i : period - 1 - i;
 }
-static __device__ HK_INL_TEXTURE vec4 sample_texture(const DeviceScene& sc, uint32_t id, vec2 uv) {
+static __device__ __forceinline__ vec4 sample_texture(const DeviceScene& sc, uint32_t id, vec2 uv) {
     uint4 ti = __ldg(&sc.texture_info[id]);
     const float4* tex = sc.texture_texels + ti.x;
     int w = (int)ti.y, h = (int)ti.z;
@@ -604,8 +577,17 @@ static __device__ HK_INL_TEXTURE vec4 sample_texture(const DeviceScene& sc, uint
     return top * (1.0f - ay) + bot * ay;
 }
 
+// The scene as a TEX = false kernel instantiation sees it (NO_TEXTURE, light.rs:141-143): texture_count == 0 as a compile-time
+// constant, which folds every `sc.texture_count != 0u` below away
+template <bool TEX>
+__device__ __forceinline__ DeviceScene scene_variant(const DeviceScene& scene) {
+    DeviceScene sc = scene;
+    if (!TEX) sc.texture_count = 0u;
+    return sc;
+}
+
 // retreive_surface, light.wgsl:730-742 (NO_TEXTURE) / 749-781
-static __device__ HK_INL_SURFACE Surface retreive_surface(const DeviceScene& sc, uint32_t material_index, vec2 uv) {
+static __device__ __forceinline__ Surface retreive_surface(const DeviceScene& sc, uint32_t material_index, vec2 uv) {
     const float4* m = reinterpret_cast<const float4*>(sc.materials + material_index);
     float4 base = ldg4(m), t0 = ldg4(m + 1), emis = ldg4(m + 2), t1 = ldg4(m + 3), t2 = ldg4(m + 4);
     Surface s;
@@ -614,22 +596,6 @@ static __device__ HK_INL_SURFACE Surface retreive_surface(const DeviceScene& sc,
     s.metallic = t1.z;
     s.occlusion = 1.0f;
     if (sc.texture_count != 0u) {
-#if HK_SURFACE_LOOP
-        // Tuning variant (off by default; validated on the emulated kernels, not yet timed): ONE inlined copy of the sampler
-        // in a rolled loop over the four texture slots instead of four copies — the same look-ups and products in the same
-        // order, 1 458 -> ~500 SASS instructions per retreive_surface site of the textured kernels (city, scene.rs)
-        const uint32_t id0 = __float_as_uint(t0.x), id1 = __float_as_uint(t1.x), id2 = __float_as_uint(t1.w), id3 = __float_as_uint(t2.z);
-#pragma unroll 1
-        for (int k = 0; k < 4; ++k) {
-            const uint32_t id = k == 0 ? id0 : (k == 1 ? id1 : (k == 2 ? id2 : id3));
-            if (id == U32_MAX) continue;
-            const vec4 t = sample_texture(sc, id, uv);
-            if (k == 0) s.base_color = s.base_color * t;
-            else if (k == 1) s.emissive = s.emissive * t;
-            else if (k == 2) s.metallic *= t.x;
-            else s.occlusion = t.x;
-        }
-#else
         uint32_t id = __float_as_uint(t0.x);
         if (id != U32_MAX) s.base_color = s.base_color * sample_texture(sc, id, uv);
         id = __float_as_uint(t1.x);
@@ -638,13 +604,12 @@ static __device__ HK_INL_SURFACE Surface retreive_surface(const DeviceScene& sc,
         if (id != U32_MAX) s.metallic *= sample_texture(sc, id, uv).x;
         id = __float_as_uint(t2.z);
         if (id != U32_MAX) s.occlusion = sample_texture(sc, id, uv).x;
-#endif
     }
     s.roughness = perceptualRoughnessToRoughness(t1.y);
     s.reflectance = t2.x;
     return s;
 }
-static __device__ HK_INL_SURFACE vec4 retreive_emissive(const DeviceScene& sc, uint32_t material_index, vec2 uv) {  // light.wgsl:744-747 / 783-793
+static __device__ __forceinline__ vec4 retreive_emissive(const DeviceScene& sc, uint32_t material_index, vec2 uv) {  // light.wgsl:744-747 / 783-793
     const float4* m = reinterpret_cast<const float4*>(sc.materials + material_index);
     vec4 emissive = f4v(ldg4(m + 2));
     if (sc.texture_count != 0u) {
@@ -675,7 +640,7 @@ __device__ __forceinline__ vec3 calculate_view(const ShadeEnv& e, vec3 world_pos
 __device__ __forceinline__ vec3 env_terms(vec3 diffuse_color, vec3 F0, float roughness, float NdotV) {
     return EnvBRDFApprox(diffuse_color, 1.0f, NdotV) + EnvBRDFApprox(F0, roughness, NdotV);
 }
-static __device__ HK_INL_SHADE vec3 env_brdf(vec3 V, vec3 N, const Surface& s) {  // light.wgsl:890-908
+static __device__ __forceinline__ vec3 env_brdf(vec3 V, vec3 N, const Surface& s) {  // light.wgsl:890-908
     vec3 base_color = xyz(s.base_color);
     float NdotV = fmax_(dot(N, V), 0.0001f);
     vec3 F0 = v3(0.16f * s.reflectance * s.reflectance * (1.0f - s.metallic)) + base_color * s.metallic;
@@ -716,11 +681,11 @@ __device__ __forceinline__ vec3 shade(const ShadeCtx& c, vec3 Lv, vec4 in_radian
     vec3 lit_radiance = (specular_light + diffuse) * xyz(in_radiance) * NoL;
     return mix(lit_radiance, c.ambient_radiance, 1.0f - in_radiance.w);
 }
-static __device__ HK_INL_SHADE vec3 shading(const ShadeEnv& e, vec3 V, vec3 N, vec3 Lv, const Surface& s, vec4 in_radiance) {
+static __device__ __forceinline__ vec3 shading(const ShadeEnv& e, vec3 V, vec3 N, vec3 Lv, const Surface& s, vec4 in_radiance) {
     return shade(make_shade_ctx(e, V, N, s), Lv, in_radiance);
 }
 // input_radiance, light.wgsl:835-867
-static __device__ HK_INL_RADIANCE vec4 input_radiance(const DeviceScene& sc, const ShadeEnv& e, vec3 ray_direction, const HitInfo& info,
+static __device__ __forceinline__ vec4 input_radiance(const DeviceScene& sc, const ShadeEnv& e, vec3 ray_direction, const HitInfo& info,
                                                bool sample_directional, uint32_t sample_emissive, bool sample_ambient) {
     vec3 radiance = v3(0.0f);
     float amb = 0.0f;
@@ -739,17 +704,14 @@ static __device__ HK_INL_RADIANCE vec4 input_radiance(const DeviceScene& sc, con
 }
 
 // hk_wide.cuh (defined there; only the WIDE instantiations of the light kernels need the definition)
-#ifndef HK_INL_WIDE
-#define HK_INL_WIDE __forceinline__
-#endif
 template <bool BOTTOM>
-static __device__ HK_INL_WIDE Hit wide_walk(const DeviceScene& sc, const Ray& ray, float max_distance, float early_distance,
+static __device__ __forceinline__ Hit wide_walk(const DeviceScene& sc, const Ray& ray, float max_distance, float early_distance,
                                             uint32_t exclude_instance, uint32_t instance);
 
 // select_light_candidate, light.wgsl:599-708.  COUNT_RAYS adds the stand-alone BLAS ray to *blas_rays.  WIDE: the BLAS ray towards
 // the light walks the mesh's 4-wide tree (hk_wide.cuh) instead of its flat array.
 template <bool COUNT_RAYS, bool WIDE = false>
-static __device__ HK_INL_SELECT LightCandidate select_light_candidate(const DeviceScene& sc, const ShadeEnv& e, vec4 rnd, vec3 position,
+static __device__ __forceinline__ LightCandidate select_light_candidate(const DeviceScene& sc, const ShadeEnv& e, vec4 rnd, vec3 position,
                                                                  vec3 normal, uint32_t instance, HitInfo& info, uint32_t& blas_rays) {
     LightCandidate cand;
     cand.max_distance = F32_MAX;
@@ -949,15 +911,8 @@ __device__ __forceinline__ void scatter_claim(const KParams& P, size_t target, i
     atomicMax(&P.planes.scatter_key[target], ((writer + 1u) << 2) | kind);
 }
 
-// 8x4-pixel tiles per warp, 4 warps per CTA (16x8 pixels): ray coherence + whole-sector plane accesses.
-// HK_CTA_WARPS (2 / 4 / 8; tuning builds): warps of a CTA sit side by side in pairs, so the CTA's tile is 16 x (2 x warps) pixels.  A CTA
-// gives its registers and warp slots back only when its slowest warp ends, and the light kernels' warps end at very different times;
-// the HK_MINB_* values are CTAs per SM and must be scaled with the CTA size by such a build.
-#ifndef HK_CTA_WARPS
-#define HK_CTA_WARPS 4
-#endif
-static_assert(HK_CTA_WARPS == 2 || HK_CTA_WARPS == 4 || HK_CTA_WARPS == 8, "tile_pixel places warps in pairs");
-constexpr int TILE_W = 16, TILE_H = 2 * HK_CTA_WARPS, CTA_THREADS = 32 * HK_CTA_WARPS;
+// 8x4-pixel tiles per warp, 4 warps per CTA side by side in pairs (16x8 pixels): ray coherence + whole-sector plane accesses.
+constexpr int TILE_W = 16, TILE_H = 8, CTA_THREADS = 128;
 #ifndef HK_MINB_INDIRECT
 #define HK_MINB_INDIRECT 8   // these kernels are latency / instruction-fetch bound and want warps, not registers.  H100 SXM, ms/frame of
                              // cornell 1080p (the benchmark) / city 4K / scene.rs 1080p (profiles/h100_tune_defaults.jsonl, "default"):

@@ -10,12 +10,6 @@
 #pragma once
 #include "hk_math.h"
 
-// Dividing by the frame size with a host-computed reciprocal (exact whenever the quotient is normal, see spatial_tap_uv); =0 restores
-// the division for A/B runs.
-#ifndef HK_SPATIAL_FAST_DIV
-#define HK_SPATIAL_FAST_DIV 1
-#endif
-
 namespace hkd {
 
 // Offset of neighbour i: radius * (cos, sin)(TAU * fract(phase + rotation + random_frame)), with the table's phase = f32(i) *
@@ -45,14 +39,9 @@ __device__ __forceinline__ hk::vec2 spatial_march_unit(hk::vec2 offset) {
 // fma(r, y, q): the correctly rounded quotient whenever it is a normal number (tools/check_runtime_division.cpp: all 2^32 inputs for
 // the benchmark extents); a subnormal quotient is absorbed by the addition to uv >= 0.5 / size
 __device__ __forceinline__ hk::vec2 spatial_tap_uv(hk::vec2 uv, hk::vec2 unit, float tap_dist, float rw, float rh, float inv_rw, float inv_rh) {
-#if HK_SPATIAL_FAST_DIV
     const float ox = hk::mul_rn(tap_dist, unit.x), oy = hk::mul_rn(tap_dist, unit.y);
     const float qx = hk::mul_rn(ox, inv_rw), qy = hk::mul_rn(oy, inv_rh);
     return hk::v2(hk::add_rn(uv.x, fmaf(fmaf(-qx, rw, ox), inv_rw, qx)), hk::add_rn(uv.y, fmaf(fmaf(-qy, rh, oy), inv_rh, qy)));
-#else
-    (void)inv_rw; (void)inv_rh;
-    return hk::v2(hk::add_rn(uv.x, hk::div_rn(hk::mul_rn(tap_dist, unit.x), rw)), hk::add_rn(uv.y, hk::div_rn(hk::mul_rn(tap_dist, unit.y), rh)));
-#endif
 }
 // The tap's pixel at upscale ratio 1: i32(tap_uv * size)
 __device__ __forceinline__ void spatial_tap_pixel(hk::vec2 tap_uv, int w, int h, int& tx, int& ty) {

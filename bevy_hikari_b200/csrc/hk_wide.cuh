@@ -18,9 +18,6 @@
 #pragma once
 #include "hk_device.cuh"
 
-#ifndef HK_INL_WIDE
-#define HK_INL_WIDE __forceinline__
-#endif
 #ifndef HK_WIDE_STACK
 #define HK_WIDE_STACK 64       // entries of 8 bytes in local memory; a scene whose trees could need more keeps the exact-order walk
 #endif
@@ -49,7 +46,7 @@ __device__ __forceinline__ bool wide_tie_first(const DeviceScene& sc, uint32_t n
 // BOTTOM = true:  traverse_bottom of instance `instance` alone (light.wgsl:400-440) — `ray` is already in its object space;
 //                 hit.instance_index is left to the caller like the reference does.
 template <bool BOTTOM>
-static __device__ HK_INL_WIDE Hit wide_walk(const DeviceScene& sc, const Ray& ray, float max_distance, float early_distance,
+static __device__ __forceinline__ Hit wide_walk(const DeviceScene& sc, const Ray& ray, float max_distance, float early_distance,
                                             uint32_t exclude_instance, uint32_t instance) {
     Hit hit;
     hit.u = 0.0f; hit.v = 0.0f; hit.distance = max_distance;

@@ -10,13 +10,7 @@
 // texture at all, light.wgsl:729-747 vs :749-793).  TEX = false instantiations see texture_count == 0 as a compile-time constant,
 // so the bilinear sampler, the wrap modes and the four texture look-ups per retreive_surface are not in the kernel at all; the
 // launchers pick them when the uploaded scene has no textures (cornell).  Values are identical by construction — the same
-// `if (sc.texture_count != 0u)` decides, at compile time instead of at run time.  -DHK_NO_TEXTURE_VARIANT=0 keeps one variant.
-#ifndef HK_NO_TEXTURE_VARIANT
-#define HK_NO_TEXTURE_VARIANT 1
-#endif
-#ifndef HK_NOVAL_VARIANT
-#define HK_NOVAL_VARIANT 1          // 0: k_direct always uses the instantiation that tests for a validation frame at run time
-#endif
+// `if (sc.texture_count != 0u)` decides, at compile time instead of at run time (scene_variant, hk_device.cuh).
 
 namespace hkd {
 
@@ -68,13 +62,6 @@ __device__ __forceinline__ Ray primary_ray(const KParams& P, const mat4& inv_vie
     }
     ray.inv_direction = 1.0f / ray.direction;
     return ray;
-}
-
-template <bool TEX>
-__device__ __forceinline__ DeviceScene scene_variant(const DeviceScene& scene) {
-    DeviceScene sc = scene;
-    if (!TEX) sc.texture_count = 0u;     // constant-folds every `sc.texture_count != 0u` below it
-    return sc;
 }
 
 template <bool COUNT, bool TEX = true, bool WIDE = false>
@@ -572,7 +559,7 @@ static dim3 grid_for(const KParams& P) {
 
 using namespace hkd;
 
-static inline bool no_texture(const KParams& P) { return HK_NO_TEXTURE_VARIANT && P.scene.texture_count == 0u; }
+static inline bool no_texture(const KParams& P) { return P.scene.texture_count == 0u; }
 // the image-exact traversal mode is a launch-wide choice (hk_set_tuning(HK_TUNE_WIDE_TRAVERSAL)) and needs the derived trees
 static inline bool wide_mode(const KParams& P, bool wide) { return wide && P.scene.wide_ready != 0u; }
 
@@ -601,7 +588,7 @@ template <bool WIDE>
 static void launch_direct(const KParams& P, bool emissive, bool count, cudaStream_t st) {
     dim3 g = grid_for(P);
     const uint32_t interval = emissive ? P.in.frame.emissive_validate_interval : P.in.frame.direct_validate_interval;
-    const bool noval = HK_NOVAL_VARIANT && !count && (P.in.frame.number % interval) != 0u;
+    const bool noval = !count && (P.in.frame.number % interval) != 0u;
     if (noval) {                         // not a validation frame: the lean instantiation
         if (no_texture(P)) {
             if (emissive) k_direct<true, false, false, true, WIDE><<<g, CTA_THREADS, 0, st>>>(P);

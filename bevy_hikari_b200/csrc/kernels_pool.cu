@@ -11,13 +11,6 @@
 
 namespace hkd {
 
-template <bool TEX>
-__device__ __forceinline__ DeviceScene pool_scene_variant(const DeviceScene& scene) {
-    DeviceScene sc = scene;
-    if (!TEX) sc.texture_count = 0u;     // constant-folds every `sc.texture_count != 0u` (NO_TEXTURE, light.rs:141-143)
-    return sc;
-}
-
 // ---------------------------------------------------------------- select_light_candidate (light.wgsl:599-708) in two halves
 // Half A: everything up to the stand-alone BLAS walk towards the sampled light point (:599-686).  `want_ray` says whether that
 // walk is needed; the caller queues it as a RAY_KIND_BLAS ray of instance `emissive_instance`.
@@ -28,7 +21,7 @@ struct LightPick {
     uint32_t emissive_instance;   // DONT_SAMPLE_EMISSIVE when no emissive is in range
     bool want_ray;
 };
-static __device__ HK_INL_SELECT LightPick light_pick(const DeviceScene& sc, const ShadeEnv& e, vec4 rnd, vec3 position, vec3 normal, uint32_t instance) {
+static __device__ __forceinline__ LightPick light_pick(const DeviceScene& sc, const ShadeEnv& e, vec4 rnd, vec3 position, vec3 normal, uint32_t instance) {
     LightPick L;
     L.rand_direction = mul(normal_basis(e.sun_dir), sample_uniform_cone_dir(rnd.z, rnd.w, e.cos_solar));
     L.ray_origin = v3(0.0f); L.ray_direction = v3(0.0f);
@@ -93,7 +86,7 @@ static __device__ HK_INL_SELECT LightPick light_pick(const DeviceScene& sc, cons
     return L;
 }
 // Half B (:687-707): the candidate and the light's HitInfo from the result of that walk.  `hit` is only read when L.want_ray.
-static __device__ HK_INL_SELECT LightCandidate light_resolve(const DeviceScene& sc, const LightPick& L, vec3 position, Hit hit, HitInfo& info) {
+static __device__ __forceinline__ LightCandidate light_resolve(const DeviceScene& sc, const LightPick& L, vec3 position, Hit hit, HitInfo& info) {
     LightCandidate cand;
     cand.max_distance = F32_MAX;
     cand.min_distance = DISTANCE_MAX;
@@ -144,7 +137,7 @@ __global__ void __launch_bounds__(POOL_THREADS, HK_POOL_MINB) kc_indirect(const 
     int x, y;
     pool_pixel(x, y, P);
     const bool in_launch = tile_active(P, x, y);
-    const DeviceScene sc = pool_scene_variant<TEX>(P.scene);
+    const DeviceScene sc = scene_variant<TEX>(P.scene);
     const hk_frame_uniform& frame = P.in.frame;
     const ShadeEnv env = make_env(P);
     const size_t idx = in_launch ? render_index(P.band, x, y) : 0;

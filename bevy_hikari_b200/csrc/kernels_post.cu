@@ -10,11 +10,6 @@
 #include "hk_tile.cuh"
 #include "hk_kernels.h"
 
-// Unconditional, batched tap loads (below); -DHK_DENOISE_BRANCHFREE=0 restores the branchy form for A/B runs.
-#ifndef HK_DENOISE_BRANCHFREE
-#define HK_DENOISE_BRANCHFREE 1
-#endif
-
 namespace hkd {
 
 __device__ __forceinline__ vec4 load16(const uint2* plane, size_t i) {
@@ -163,11 +158,9 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_DENOISE) k_denoise(const 
         // tap order of denoise.wgsl:252-268
         const int OX[8] = {-1, 0, 1, -1, 1, -1, 0, 1};
         const int OY[8] = {-1, -1, -1, 0, 0, 1, 1, 1};
-#if HK_DENOISE_BRANCHFREE
-        // Default (-DHK_DENOISE_BRANCHFREE=0 restores the branchy form): every tap's
-        // loads are unconditional — out-of-frame taps read a clamped, valid address — and go through the read-only path, so
-        // nothing but register pressure keeps the compiler from issuing the loads of later taps during the arithmetic of
-        // earlier ones; only the accumulation is predicated.  Same operations on the same values for every tap that counts.
+        // Every tap's loads are unconditional (out-of-frame taps read a clamped, valid address) and go through the read-only path, so
+        // nothing but register pressure keeps the compiler from issuing the loads of later taps during the arithmetic of earlier
+        // ones; only the accumulation is predicated.  Same operations on the same values for every tap that counts.
 #pragma unroll
         for (int t = 0; t < 8; ++t) {
             const int ox = OX[t], oy = OY[t];
@@ -181,43 +174,6 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_DENOISE) k_denoise(const 
             for (int sgl = 0; sgl < 3; ++sgl) bits[sgl] = (sgl < signals) ? __ldg(&P.planes.dn_internal[LEVEL][sgl][sidx]) : make_uint2(0u, 0u);
             const vec3 sample_normal = f4xyz(sample_geometry);
             const float sample_depth = sample_geometry.w;
-            const float w_normal = pow16(fmax_(0.0f, dot(normal, sample_normal)));
-            const float w_depth = exp_((-fabsf(depth - sample_depth)) / (fabsf(dot(depth_gradient, v2((float)ox, (float)oy))) + 0.01f));
-            const float w_instance = fmax_(0.0f, 1.0f - fabsf(instance - sample_instance));
-            const float w_geometry = w_normal * w_depth * w_instance;
-            const float k = kernel_at(P, oy + 1, ox + 1);
-#pragma unroll
-            for (int sgl = 0; sgl < 3; ++sgl) {
-                if (sgl >= signals) continue;
-                SignalAcc& a = acc[sgl];
-                uvec2 q; q.x = bits[sgl].x; q.y = bits[sgl].y;
-                vec3 irr = xyz(unpack_rgba16f(q));
-                float sample_luminance = luminance(irr);
-                float w_luminance = exp_((-fabsf(a.lum - sample_luminance)) / a.lum_denominator);
-                float w = clampf(w_geometry * w_luminance, 0.0f, 1.0f) * k;
-                if (valid && !bad3(irr)) {
-                    a.sum_irradiance = a.sum_irradiance + irr * w;
-                    a.sum_w += w;
-                    if (sgl != 0) {
-                        a.ff_moment_1 += sample_luminance;
-                        a.ff_moment_2 += sample_luminance * sample_luminance;
-                        a.ff_count += 1.0f;
-                    }
-                }
-            }
-        }
-#else
-#pragma unroll
-        for (int t = 0; t < 8; ++t) {
-            const int ox = OX[t], oy = OY[t];
-            const int sx = x + ox * STEP, sy = y + oy * STEP;
-            if (sx < 0 || sy < 0 || sx >= P.band.RW || sy >= P.band.RH) continue;
-            const size_t sidx = render_index(P.band, sx, sy);
-            // geometric weights: once per tap for all signals
-            const float4 sample_geometry = P.planes.dn_geometry[sidx];
-            const vec3 sample_normal = f4xyz(sample_geometry);
-            const float sample_depth = sample_geometry.w;
-            const float sample_instance = P.planes.dn_instance[sidx];
             const float w_normal = pow16(fmax_(0.0f, dot(normal, sample_normal)));                                       // :44-47
             const float w_depth = exp_((-fabsf(depth - sample_depth)) / (fabsf(dot(depth_gradient, v2((float)ox, (float)oy))) + 0.01f));  // :50-53
             const float w_instance = fmax_(0.0f, 1.0f - fabsf(instance - sample_instance));                              // :63-65
@@ -227,22 +183,22 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_DENOISE) k_denoise(const 
             for (int sgl = 0; sgl < 3; ++sgl) {
                 if (sgl >= signals) continue;
                 SignalAcc& a = acc[sgl];
-                vec3 irr = xyz(load16(P.planes.dn_internal[LEVEL][sgl], sidx));
-                if (bad3(irr)) continue;
+                uvec2 q; q.x = bits[sgl].x; q.y = bits[sgl].y;
+                vec3 irr = xyz(unpack_rgba16f(q));
                 float sample_luminance = luminance(irr);
                 float w_luminance = exp_((-fabsf(a.lum - sample_luminance)) / a.lum_denominator);                       // :56-61
                 float w = clampf(w_geometry * w_luminance, 0.0f, 1.0f) * k;
-                a.sum_irradiance = a.sum_irradiance + irr * w;
-                a.sum_w += w;
-                if (sgl != 0) {  // FIREFLY_FILTERING: emissive + indirect only (post_process.rs:1193-1197)
-                    a.ff_moment_1 += sample_luminance;
-                    a.ff_moment_2 += sample_luminance * sample_luminance;
-                    a.ff_count += 1.0f;
+                if (valid && !bad3(irr)) {
+                    a.sum_irradiance = a.sum_irradiance + irr * w;
+                    a.sum_w += w;
+                    if (sgl != 0) {  // FIREFLY_FILTERING: emissive + indirect only (post_process.rs:1193-1197)
+                        a.ff_moment_1 += sample_luminance;
+                        a.ff_moment_2 += sample_luminance * sample_luminance;
+                        a.ff_count += 1.0f;
+                    }
                 }
             }
         }
-
-#endif
 
         vec4 albedo = v4(1.0f);
         if (LEVEL == 3) albedo = load16(P.planes.albedo, gidx);

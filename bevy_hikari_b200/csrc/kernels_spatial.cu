@@ -4,15 +4,6 @@
 // BVH stay on exact arithmetic.  The exact build compiles it like everything else and is bit-identical to the oracle.
 #include "hk_tile.cuh"
 #include "hk_kernels.h"
-
-#ifndef HK_NO_TEXTURE_VARIANT
-#define HK_NO_TEXTURE_VARIANT 1
-#endif
-// Requesting a neighbour's reservoir together with its depth (=0 restores the two-step load for A/B runs).  The depth march's
-// division by the frame size, HK_SPATIAL_FAST_DIV, is a switch of hk_spatial_taps.cuh.
-#ifndef HK_SPATIAL_EAGER_LOAD
-#define HK_SPATIAL_EAGER_LOAD 1
-#endif
 #include "hk_spatial_taps.cuh"
 
 // CTAs of 256 threads per SM of the tiled kernel: 74 KB of shared memory each for the indirect pipeline (at most 3 fit), 32 KB for the
@@ -23,24 +14,8 @@
 #ifndef HK_SPATIAL_TILED_MINB_EMISSIVE
 #define HK_SPATIAL_TILED_MINB_EMISSIVE 2
 #endif
-// kc_spatial stages its tiles only when one of its pixels is a surface pixel (=0: every CTA stages them, for A/B runs)
-#ifndef HK_SPATIAL_SKIP_EMPTY_TILES
-#define HK_SPATIAL_SKIP_EMPTY_TILES 1
-#endif
-// Surviving neighbours whose gathers kc_spatial keeps in flight ahead of the one it merges.  Each holds 12 registers: 2 spills at the
-// 127-register cap of 2 CTAs/SM and was slower on the H100 (cornell 1080p)
-#ifndef HK_SPATIAL_GATHER_AHEAD
-#define HK_SPATIAL_GATHER_AHEAD 1
-#endif
 
 namespace hkd {
-
-template <bool TEX>
-__device__ __forceinline__ DeviceScene scene_variant(const DeviceScene& scene) {
-    DeviceScene sc = scene;
-    if (!TEX) sc.texture_count = 0u;     // constant-folds every `sc.texture_count != 0u` below it
-    return sc;
-}
 
 // ----------------------------------------------------------------------------------- P4: spatial_reuse
 // light.wgsl:1500-1684.  The reference's 8x8 workgroup cache holds unpack(reservoir_buffer[..]) of this dispatch's
@@ -110,10 +85,8 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_SPATIAL) k_spatial(const 
         // (size + 0.5) / size >= 1 + 2^-23 survive rounding), so the two IEEE divisions per neighbour are not needed.
         if (sx < 0 || sy < 0 || sx >= P.band.RW || sy >= P.band.RH) continue;
         const size_t sidx = render_index(P.band, sx, sy);
-#if HK_SPATIAL_EAGER_LOAD
-        // Default (-DHK_SPATIAL_EAGER_LOAD=0 restores the two-step form): the neighbour's reservoir
-        // is requested together with its depth instead of after the depth test, so a neighbour exposes one load latency
-        // instead of two; rejected neighbours cost 64 bytes of L1/L2 traffic more.
+        // The neighbour's reservoir is requested together with its depth instead of after the depth test, so a neighbour exposes
+        // one load latency instead of two; rejected neighbours cost 64 bytes of L1/L2 traffic more.
         const float* depth_ptr = &P.planes.pos_depth[light_gbuffer_index(P, sx, sy, sidx)].w;
         const float sample_depth = __ldg(depth_ptr);
         PackedQuarters packed;
@@ -122,12 +95,6 @@ __global__ void __launch_bounds__(CTA_THREADS, HK_MINB_SPATIAL) k_spatial(const 
         float depth_ratio = depth / sample_depth;
         if (depth_ratio < 0.9f || depth_ratio > 1.1f) continue;
         q = unpack_reservoir(packed);
-#else
-        const float sample_depth = P.planes.pos_depth[light_gbuffer_index(P, sx, sy, sidx)].w;
-        float depth_ratio = depth / sample_depth;
-        if (depth_ratio < 0.9f || depth_ratio > 1.1f) continue;
-        q = unpack_reservoir(load_quarters(B.reservoir, sidx));
-#endif
         bool normal_miss = dot(s.visible_normal, q.s.visible_normal) < 0.866f;
         if (q.count < F32_EPSILON || normal_miss) continue;
         vec3 sample_direction = normalize(xyz(q.s.sample_position) - xyz(s.visible_position));
@@ -234,22 +201,11 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
     // tile origin in frame coordinates, and in plane (allocation) coordinates for the copy engine
     const int px0 = tile_origin_x(P.col_lo + (int)blockIdx.x * POOL_TILE_W - R - P.band.ax0);       // plane column of the tile's first cell
     const int tx0 = px0 + P.band.ax0, ty0 = P.row_lo + (int)blockIdx.y * POOL_TILE_H - R;
-    auto stage_tiles = [&]() {
-        mbar_expect_tx(s_bar, ST::TX_BYTES);
-        tile_load_2d(s_depth, &depth_map, px0, ty0 - P.band.a0, s_bar);
-        tile_load_2d(s_q3, &q3_map, 4 * px0, ty0 - P.band.a0, s_bar);      // the plane as rows of u32: 4 per pixel
-        mbar_complete_emulated(s_bar);
-    };
-    if (threadIdx.x == 0) {
-        mbar_init(s_bar, 1u);
-        if (!HK_SPATIAL_SKIP_EMPTY_TILES) stage_tiles();
-    }
-    if (!HK_SPATIAL_SKIP_EMPTY_TILES) __syncthreads();      // the barrier is initialised before anybody waits on it
+    if (threadIdx.x == 0) mbar_init(s_bar, 1u);
 
     int x, y;
     pool_pixel(x, y, P);
     const bool in_launch = tile_active(P, x, y);
-    // everything that does not need the tiles first: the copies run meanwhile
     const DeviceScene sc = scene_variant<TEX>(P.scene);
     const hk_frame_uniform& frame = P.in.frame;
     const size_t idx = in_launch ? render_index(P.band, x, y) : 0;
@@ -264,16 +220,18 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
         store_quarters(Bf.spatial_reservoir, idx, pack_reservoir(unpack_reservoir(own)));
         P.planes.render[SIGNAL][idx] = make_uint2(0u, 0u);
     }
-#if HK_SPATIAL_SKIP_EMPTY_TILES
     // A CTA of background pixels only (around the model) needs no neighbourhood: it stages nothing and leaves at once.  Otherwise
     // its background threads leave without waiting: the surface threads wait for the copies before the CTA's memory can go away.
     if (!__syncthreads_or(surface_pixel)) return;       // (also orders the barrier's initialisation before any wait on it)
-    if (threadIdx.x == 0) stage_tiles();
+    if (threadIdx.x == 0) {
+        mbar_expect_tx(s_bar, ST::TX_BYTES);
+        tile_load_2d(s_depth, &depth_map, px0, ty0 - P.band.a0, s_bar);
+        tile_load_2d(s_q3, &q3_map, 4 * px0, ty0 - P.band.a0, s_bar);      // the plane as rows of u32: 4 per pixel
+        mbar_complete_emulated(s_bar);
+    }
     if (!surface_pixel) return;
-#else
-    if (!surface_pixel) { mbar_wait(s_bar, 0u); return; }      // (every thread observes the copies before the CTA's memory can go away)
-#endif
 
+    // everything that does not need the tiles first: the copies run meanwhile
     Reservoir r = unpack_reservoir(own);
     const ShadeEnv env = make_env(P);
     const vec3 position = f4xyz(pd);
@@ -369,14 +327,17 @@ __global__ void __launch_bounds__(POOL_THREADS, EMISSIVE_LIT ? HK_SPATIAL_TILED_
         g.q0 = __ldg(&Bf.reservoir.q[0][sidx]); g.q1 = __ldg(&Bf.reservoir.q[1][sidx]); g.q2 = __ldg(&Bf.reservoir.q[2][sidx]);
         return g;
     };
-    Gather ahead[HK_SPATIAL_GATHER_AHEAD + 1];
+    // One survivor's gathers in flight ahead of the one being merged.  Each holds 12 registers: two ahead spilled at the 127-register
+    // cap of 2 CTAs/SM and was slower on the H100 (cornell 1080p)
+    constexpr int GATHER_AHEAD = 1;
+    Gather ahead[GATHER_AHEAD + 1];
 #pragma unroll
-    for (int k = 0; k <= HK_SPATIAL_GATHER_AHEAD; ++k) ahead[k] = gather_next();
+    for (int k = 0; k <= GATHER_AHEAD; ++k) ahead[k] = gather_next();
     while (ahead[0].valid) {
         const Gather cur = ahead[0];
 #pragma unroll
-        for (int k = 0; k < HK_SPATIAL_GATHER_AHEAD; ++k) ahead[k] = ahead[k + 1];
-        ahead[HK_SPATIAL_GATHER_AHEAD] = gather_next();
+        for (int k = 0; k < GATHER_AHEAD; ++k) ahead[k] = ahead[k + 1];
+        ahead[GATHER_AHEAD] = gather_next();
         PackedQuarters packed;
         packed.q0 = cur.q0; packed.q1 = cur.q1; packed.q2 = cur.q2; packed.q3 = s_q3[cur.cell];
         q = unpack_reservoir(packed);
@@ -418,7 +379,7 @@ static dim3 grid_for(const KParams& P) {
 
 using namespace hkd;
 
-static inline bool no_texture(const KParams& P) { return HK_NO_TEXTURE_VARIANT && P.scene.texture_count == 0u; }
+static inline bool no_texture(const KParams& P) { return P.scene.texture_count == 0u; }
 
 template <bool EMISSIVE_LIT, bool TEX>
 static void launch_tiled(const KParams& P, const TileMap& depth_map, const TileMap& q3_map, const SpatialTable& table, cudaStream_t st) {

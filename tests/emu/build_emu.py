@@ -27,7 +27,7 @@ CPP = ["hikari.cpp", "hikari_capi.cpp", "gltf_ingest.cpp", "hikari_plugin.cpp", 
 CXX = os.environ.get("HK_CXX", "/usr/bin/g++")
 FLAGS = ["-O2", "-march=x86-64-v3", "-ffp-contract=off", "-fno-fast-math", "-fopenmp", "-fPIC", "-std=c++17", "-w",
          "-I" + os.path.join(HERE, "include"), "-I" + SRC, "-I" + HOST, "-I" + os.path.join(ROOT, "include")] + \
-        os.environ.get("HK_EMU_EXTRA", "").split()      # e.g. -DHK_DENOISE_BRANCHFREE=1: validate a tuning variant's logic
+        os.environ.get("HK_EMU_EXTRA", "").split()      # e.g. -DHK_WIDE_STACK=32: validate a tuning variant's logic
 if ASAN:
     FLAGS = [f for f in FLAGS if f != "-O2"] + ["-O1", "-g1", "-fno-var-tracking-assignments", "-fsanitize=address", "-fno-omit-frame-pointer"]
 if ALIGN:

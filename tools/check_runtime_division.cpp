@@ -1,4 +1,4 @@
-// Exhaustive check of the runtime-constant exact division used by the -DHK_SPATIAL_FAST_DIV=1 variant:
+// Exhaustive check of the runtime-constant exact division used by spatial_tap_uv (bevy_hikari_b200/csrc/hk_spatial_taps.cuh):
 //     q = x * y;  r = fma(-q, C, x);  result = fma(r, y, q)      with y = RN(1 / C) computed once on the host
 // against IEEE x / C for EVERY float x (all 2^32 bit patterns) and a list of image extents C.
 // build: g++ -O2 -march=x86-64-v3 -ffp-contract=off -fopenmp tools/check_runtime_division.cpp -o /tmp/divcheck/check

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""SASS size of the light kernels under a set of inlining-policy flags (no GPU needed).
-usage: tools/code_size.py [-DHK_INL_TRAVERSE=__noinline__ ...]
+"""SASS size of the light kernels under a set of extra nvcc flags (no GPU needed).
+usage: tools/code_size.py [-DHK_MINB_INDIRECT=12 ...]
 Compiles bevy_hikari_b200/csrc/kernels_light.cu with the build's flags + the given ones into a scratch object and prints
 instructions / KB / registers / spill bytes per kernel."""
 import collections

@@ -1,8 +1,7 @@
 #!/bin/bash
 # Round 2, call 16 (1 GPU, 8.6 GPU-minutes left):
 #   1. the whole device suite on the tree with the reference's SMAA / TAA output extents (Band::OW / OH) and the five upscaler fixtures;
-#   2. A/B of the CTA size of the per-pixel kernels (HK_CTA_WARPS = 2 / 4 / 8 at the same registers and warps per SM: a CTA frees its warp
-#      slots only when its slowest warp ends) and of the L1 preference (HK_TUNE_PREFER_L1), on the three scenes.
+#   2. the default on the three scenes.
 mkdir -p gpurun_out
 O=gpurun_out
 T=r2c16
@@ -29,13 +28,9 @@ run() {  # name lib-or-empty config steps warmup
   timeout 60 python bench.py $libarg --config $3 --steps $4 --warmup $5 --no-cpu-baseline 2> $O/${T}_$1_$3.err | grep "^{" > $O/${T}_$1_$3.json
   short $O/${T}_$1_$3.json $1
 }
-echo "== 2. variants ($(left) s left)"
+echo "== 2. default ($(left) s left)"
 for cfg in "cornell_1080p 16 4" "scene_1080p 8 3" "city_4k 6 3"; do
   set -- $cfg
   [ $(left) -gt 20 ] && run default "" $1 $2 $3
-  [ $(left) -gt 20 ] && HK_TUNE_PREFER_L1=1 run default_l1 "" $1 $2 $3
-  for v in w2 w2d24 w8; do
-    [ $(left) -gt 20 ] && [ -f bevy_hikari_b200/variants/$v.so ] && run $v bevy_hikari_b200/variants/$v.so $1 $2 $3
-  done
 done
 echo "== done after $(( $(date +%s) - START )) s"

@@ -1,7 +1,7 @@
 #!/bin/bash
-# Round 2, ninth gpurun call (1 GPU, benches only): is the instruction cache the lever on the light kernels?  The reference-order walk
-# outlined into ONE copy per kernel (-DHK_INL_TRAVERSE=__noinline__; round 1 timed it on cornell only) and the CTAs-per-SM knob, on the
-# deep scenes where the walk dominates; the new default (primary rays on the 4-wide trees) as the baseline.
+# Round 2, ninth GPU call (1 GPU, benches only): is the instruction cache the lever on the light kernels?  The CTAs-per-SM knob
+# (HK_MINB_* variants built by tools/build_variants.py), on the deep scenes where the walk dominates; the new default (primary rays on
+# the 4-wide trees) as the baseline.
 mkdir -p gpurun_out
 O=gpurun_out
 T=r2c11
